@@ -71,6 +71,25 @@ def test_argument_validation_and_loud_failure_without_device():
         assert "no CPU fallback" in str(e.value)
 
 
+def test_level_histogram_seam_validates_without_device():
+    """Both entry points of the level-histogram seam refuse null arguments before touching a device."""
+    L = ydf_b200.lib()
+    assert C.sizeof(_capi.HistPlan) == 24   # sizeof(ygg_hist_plan)
+    p = _capi.HistPlan()
+    assert L.ygg_debug_hist_plan(None, 0, C.byref(p)) == 1
+    assert "null" in L.ygg_last_error().decode()
+    g = np.zeros(4, np.float32)
+    slots = np.zeros(4, np.int32)
+    s = np.zeros(256, np.uint64)
+    c = np.zeros(256, np.uint32)
+    sc = np.zeros(2, np.float32)
+    P = _capi.ptr
+    assert L.ygg_debug_level_histogram(None, 0, None, P(g, C.c_float), None, P(slots, C.c_int32), 1, P(s, C.c_uint64),
+                                       P(c, C.c_uint32), None, P(sc, C.c_float)) == 1
+    assert L.ygg_debug_level_histogram(None, 0, C.byref(p), None, None, None, 1, None, None, None, None) == 1
+    assert not s.any() and not c.any() and not sc.any()
+
+
 def test_learner_rejects_options_outside_the_path():
     L = ydf_b200.GradientBoostedTreesLearner
     # exact splitter (discretize_numerical_columns=False, the reference's default): reproduced with one bucket per distinct

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import ydf_b200
+from tests.util import level_histogram_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -78,4 +79,13 @@ def test_full_size_properties(data):
         P = 2.0 ** np.ceil(np.log2(np.abs(g).max()))
         assert np.all(np.abs(s - want_s) <= want_c * P * 2.0 ** -24 + 1e-9)
         assert c.sum() == n
+    # ... and run as training runs it (the handle's root plan), against the integer reference: exact
+    slots = np.zeros(n, np.int32)
+    s, c, _, (P, _) = gbt2.level_histogram(0, g, slots, 1)
+    want_s, want_c, _, want_P = level_histogram_ref(bins, slots, 1, g, features=(0, 199))
+    assert P == want_P
+    for i, f in enumerate((0, 199)):
+        np.testing.assert_array_equal(c[0, f].astype(np.int64), want_c[0, i])
+        np.testing.assert_array_equal(s[0, f].astype(np.int64), want_s[0, i])
+        assert c[0, f].sum() == n
     gbt2.close(); ds2.close()

@@ -8,7 +8,7 @@ import pytest
 
 import ydf_b200
 from oracle import oracle as O
-from tests.util import compare_trees, first_divergence, synth
+from tests.util import compare_trees, first_divergence, level_histogram_ref, synth
 
 pytestmark = pytest.mark.gpu
 
@@ -100,6 +100,14 @@ def test_histogram_matches_numpy(n):
         # 24-bit fixed point: |err| <= count * P * 2^-24
         P = 2.0 ** np.ceil(np.log2(np.abs(g).max()))
         assert np.all(np.abs(s - want_s) <= want_c * P * 2.0 ** -24 + 1e-12)
+    # the raw integer planes of every feature, exactly: the rows of node 1 in the one slot of level 1 (sibling
+    # subtraction: one directly accumulated node), accumulated with the handle's own plan of that level
+    slots = np.where(node_of_row == 1, 0, -1).astype(np.int32)
+    s, c, _, (P, _) = gbt.level_histogram(1, g, slots, 1)
+    want_s, want_c, _, want_P = level_histogram_ref(bins, slots, 1, g)
+    assert P == want_P
+    np.testing.assert_array_equal(c.astype(np.int64), want_c)
+    np.testing.assert_array_equal(s.astype(np.int64), want_s)
 
 
 CASES = [

@@ -161,6 +161,70 @@ def first_divergence(trees_a, trees_b, prune_noise=None, present_in=None, **kw):
     return None, []
 
 
+def pow2_cover(m):
+    """Smallest power of two >= m (a normal float32 >= 0); 1 for m == 0: the histogram scale P of max|g| = m."""
+    m = np.float32(m)
+    if m == 0:
+        return np.float32(1.0)
+    f, e = np.frexp(m)          # m = f * 2^e, f in [0.5, 1)
+    return np.float32(np.ldexp(np.float32(1.0), int(e) - 1 if f == 0.5 else int(e)))
+
+
+def quantize_q24(g, P):
+    """Biased 24-bit gradient code: clip(rint(g * 2^23 / P) + 2^23, 0, 2^24 - 1).  Exact in float32: the scale is a power
+    of two, so g * 2^23 / P is the exact product, and integers up to 2^24 are float32 values."""
+    g = np.asarray(g, np.float32)
+    t = np.rint(g * np.float32(2.0 ** 23 / float(P))) + np.float32(2.0 ** 23)
+    return np.clip(t, 0, 2 ** 24 - 1).astype(np.int64)
+
+
+def quantize_second(v, V):
+    """Hessian / weight code: min(rint(v * 2^24 / V), 2^24), 2^24 inclusive (v == V stays exact)."""
+    v = np.asarray(v, np.float32)
+    return np.minimum(np.rint(v * np.float32(2.0 ** 24 / float(V))), np.float32(2.0 ** 24)).astype(np.int64)
+
+
+def level_histogram_ref(bins, slot_of_row, n_slots, g, second=None, V=None, features=None):
+    """Integer reference of one level's slot histograms: per (slot, feature, bin) the sum of the biased gradient codes,
+    the row count and (with `second`, quantised against the power of two V) the sum of the second-plane codes.
+    -> (sum, count, second sum or None, P), int64 arrays of shape [n_slots, len(features), 256]."""
+    features = range(bins.shape[0]) if features is None else features
+    slot_of_row = np.asarray(slot_of_row)
+    P = pow2_cover(np.abs(np.asarray(g, np.float32)).max() if len(g) else 0)
+    q = quantize_q24(g, P)
+    hq = quantize_second(second, V) if second is not None else None
+    act = slot_of_row >= 0
+    assert (int(act.sum()) + 1) * 2 ** 24 < 2 ** 53
+    s = slot_of_row[act].astype(np.int64) * 256
+    qa = q[act]
+    ha = hq[act] if hq is not None else None
+    shape = (n_slots, len(features), 256)
+    out_s, out_c = np.zeros(shape, np.int64), np.zeros(shape, np.int64)
+    out_h = np.zeros(shape, np.int64) if hq is not None else None
+    for i, f in enumerate(features):
+        key = s + bins[f][act]
+        out_c[:, i, :] = np.bincount(key, minlength=n_slots * 256).reshape(n_slots, 256)
+        # float64 accumulation of integers < 2^24 is exact while every partial sum stays below 2^53 (asserted above)
+        out_s[:, i, :] = np.bincount(key, weights=qa, minlength=n_slots * 256).astype(np.int64).reshape(n_slots, 256)
+        if hq is not None:
+            out_h[:, i, :] = np.bincount(key, weights=ha, minlength=n_slots * 256).astype(np.int64).reshape(n_slots, 256)
+    return out_s, out_c, out_h, P
+
+
+def chunk_max_count(bins, chunk_blocks, features=None, block_rows=8192):
+    """Largest number of rows of one aligned chunk of `chunk_blocks` row blocks that share a bin of one feature."""
+    features = range(bins.shape[0]) if features is None else features
+    n = bins.shape[1]
+    n_blocks = (n + block_rows - 1) // block_rows
+    n_chunks = (n_blocks + chunk_blocks - 1) // chunk_blocks
+    chunk_of_row = np.arange(n) // (block_rows * chunk_blocks)
+    best = 0
+    for f in features:
+        c = np.bincount(chunk_of_row * 256 + bins[f], minlength=n_chunks * 256)
+        best = max(best, int(c.max()))
+    return best
+
+
 def predict_raw(trees, initial_prediction, bins):
     """Sum of the leaves reached by every column of `bins` ([F, n] bucket / dictionary codes) — numpy walk of
     ydf_b200.NODE_DTYPE trees (DiscretizedHigher and Contains conditions)."""

@@ -43,6 +43,17 @@ assert NODE_DTYPE.itemsize == 112  # sizeof(ygg_node), include/ygg_b200.h
 FEATURE_DISCRETIZED_NUMERICAL = 0
 FEATURE_CATEGORICAL = 1
 
+HIST_ROOT_SUM, HIST_PACKED, HIST_SHARED, HIST2 = 0, 1, 2, 3   # enum ygg_hist_mode
+
+
+class HistPlan(C.Structure):
+    """One level's k_hist / k_hist2 launch (ygg_hist_plan)."""
+    _fields_ = [("mode", C.c_int32), ("group", C.c_int32), ("hist2_tiles", C.c_int32), ("chunk_blocks", C.c_int32),
+                ("slot_window", C.c_int32), ("grid", C.c_int32)]
+
+    def __repr__(self):
+        return "HistPlan(%s)" % ", ".join("%s=%d" % (k, getattr(self, k)) for k, _ in self._fields_)
+
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p)
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p)
 REDUCESCATTER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p)
@@ -55,7 +66,7 @@ EXPORTS = [
     "ygg_merge_shard_best", "ygg_gbt_initial_prediction",
     "ygg_gbt_train", "ygg_gbt_train_timed", "ygg_gbt_step", "ygg_gbt_sync", "ygg_gbt_num_trees", "ygg_gbt_get_tree",
     "ygg_gbt_train_loss", "ygg_gbt_get_predictions", "ygg_gbt_set_predictions", "ygg_gbt_predict",
-    "ygg_tree_train_on_gradients", "ygg_debug_histogram", "ygg_partition_rows",
+    "ygg_tree_train_on_gradients", "ygg_debug_hist_plan", "ygg_debug_level_histogram", "ygg_partition_rows",
     "ygg_gbt_set_profiling", "ygg_gbt_get_profile", "ygg_gbt_save_ydf",
     "ygg_discretize_boundaries", "ygg_discretize_encode", "ygg_model_write_ydf",
     "ygg_validation_split_mask", "ygg_dataset_split_rows", "ygg_gbt_set_validation_i32",
@@ -361,6 +372,7 @@ class Gbt:
         """Example weights of the training rows (before set_labels): weighted histograms, leaves, losses, initial predictions."""
         w = np.ascontiguousarray(weights, dtype=np.float32)
         check(lib().ygg_gbt_set_weights_f32(self.handle, ptr(w, C.c_float), C.c_int64(len(w))))
+        self._weighted = True
 
     def set_validation(self, dataset, labels, weights=None):
         """Held-out rows (same features / binning): validation loss per iteration + cfg.early_stopping."""
@@ -395,6 +407,7 @@ class Gbt:
     def set_feature_shard(self, begin, end, rank, world, allgather=None):
         """allgather: a Comm (NCCL, called from C++ without touching Python), or a Python callable
         allgather(send_ptr, recv_ptr, nbytes, stream_ptr) -> int, called once per tree level."""
+        self._hist_features = (int(begin), int(end))
         if isinstance(allgather, Comm):
             self._comm = allgather
             fn = C.cast(lib().ygg_comm_allgather, ALLGATHER_FN)
@@ -556,16 +569,58 @@ class Gbt:
                                                 C.byref(n)))
         return out[:n.value].copy()
 
-    def debug_histogram(self, g, node_of_row, node, feature):
+    def hist_plan(self, level):
+        """The k_hist / k_hist2 launch the handle runs at tree level `level` (HistPlan)."""
+        p = HistPlan()
+        check(lib().ygg_debug_hist_plan(self.handle, C.c_int32(level), C.byref(p)))
+        return p
+
+    def level_histogram(self, level, g, slot_of_row, n_slots, second=None, plan=None):
+        """Raw integer histograms of one tree level run by the training code (ygg_debug_level_histogram): rows with
+        slot_of_row[r] = s >= 0 go to slot s.  -> (sum u64, count u32, second-plane sum u64 or None) of shape
+        [n_slots, features histogrammed by this handle, 256], and (P, V): the scales of g and of the second plane."""
         g = np.ascontiguousarray(g, dtype=np.float32)
-        nor = np.ascontiguousarray(node_of_row, dtype=np.int32)
+        slots = np.ascontiguousarray(slot_of_row, dtype=np.int32)
+        v = None if second is None else np.ascontiguousarray(second, dtype=np.float32)
+        lo, hi = self.hist_features()
+        shape = (int(n_slots), hi - lo, 256)
+        s = np.zeros(shape, np.uint64)
+        c = np.zeros(shape, np.uint32)
+        s2 = None if v is None else np.zeros(shape, np.uint64)
+        scales = np.zeros(2, np.float32)
+        check(lib().ygg_debug_level_histogram(self.handle, C.c_int32(level), None if plan is None else C.byref(plan),
+                                              ptr(g, C.c_float), ptr(v, C.c_float), ptr(slots, C.c_int32),
+                                              C.c_int32(n_slots), ptr(s, C.c_uint64), ptr(c, C.c_uint32),
+                                              ptr(s2, C.c_uint64), ptr(scales, C.c_float)))
+        return s, c, s2, (float(scales[0]), float(scales[1]))
+
+    def has_second_plane(self):
+        """True when the handle accumulates a second histogram plane: hessians (hessian gain with a logit loss) or
+        example weights (the caller's or GOSS's)."""
+        weighted = getattr(self, "_weighted", False) or self.cfg.goss_alpha > 0 or self.cfg.goss_beta > 0
+        logit = self.cfg.loss in (0, 2)   # binomial / multinomial log-likelihood
+        return bool((self.cfg.use_hessian_gain and (logit or weighted)) or weighted)
+
+    def debug_histogram(self, g, node_of_row, node, feature):
+        """Histogram of feature `feature` over the rows with node_of_row == node, dequantised: (sum of the quantised
+        gradients per bin as float64, row count per bin), num_bins[feature] entries each.  A view of level_histogram: one
+        slot at the root level, accumulated by the shared layout (exact for any rows) at the root's chunk size and grid."""
+        lo, hi = self.hist_features()
+        if not lo <= feature < hi:
+            raise ValueError(f"feature {feature} outside the histogrammed features [{lo}, {hi})")
+        slots = np.where(np.asarray(node_of_row) == node, 0, -1).astype(np.int32)
+        root = self.hist_plan(0)
+        p = HistPlan(HIST_SHARED, 1, 0, root.chunk_blocks, 0, root.grid)
+        second = np.zeros(len(slots), np.float32) if self.has_second_plane() else None
+        s, c, _, (P, _) = self.level_histogram(0, g, slots, 1, second=second, plan=p)
         nb = int(self.dataset.num_bins[feature])
-        s = np.zeros(nb, dtype=np.float64)
-        c = np.zeros(nb, dtype=np.int64)
-        check(lib().ygg_debug_histogram(self.handle, ptr(g, C.c_float), ptr(nor, C.c_int32),
-                                        C.c_int32(node), C.c_int32(feature), ptr(s, C.c_double),
-                                        ptr(c, C.c_int64)))
-        return s, c
+        cnt = c[0, feature - lo, :nb].astype(np.int64)
+        raw = s[0, feature - lo, :nb].astype(np.int64) - cnt * 2 ** 23   # exact: |raw| <= rows * 2^23 < 2^63
+        return raw.astype(np.float64) * (P / 2.0 ** 23), cnt
+
+    def hist_features(self):
+        """[begin, end) of the features this handle histograms (its feature shard, or all features)."""
+        return getattr(self, "_hist_features", (0, self.dataset.n_features))
 
     def set_profiling(self, enabled=True):
         check(lib().ygg_gbt_set_profiling(self.handle, C.c_int32(int(enabled))))

@@ -335,22 +335,24 @@ struct LevelBuf {
 };
 // Layout of the level buffer for `slots` histogram slots and `n_stats_nodes` node statistics:
 // per chunk [sum u64 | hsum u64 (hessian) | cnt u32, padded to u64 | stats 3 u64 per node].
-LevelBuf level_buf(const ygg_gbt* h, int slots, int n_stats_nodes) {
+// `base`: the buffer the layout is laid over (null: the handle's level buffer).
+LevelBuf level_buf(const ygg_gbt* h, int slots, int n_stats_nodes, unsigned long long* base = nullptr) {
   LevelBuf lb;
   const int f_hist = h->hist_f_end - h->hist_f_begin;
   lb.W = h->scatter ? h->world : 1;
   lb.f_chunk = (f_hist + lb.W - 1) / lb.W;
   const size_t B = static_cast<size_t>(slots) * lb.f_chunk * kMaxBins;
-  lb.sum = h->d_level_buf;
+  if (base == nullptr) base = h->d_level_buf;
+  lb.sum = base;
   unsigned long long* p = lb.sum + B;
   lb.hsum = nullptr;
   if (hist_hess(h)) { lb.hsum = p; p += B; }
   lb.cnt = reinterpret_cast<uint32_t*>(p);
   p += (B + 1) / 2;
   lb.stats = p;
-  lb.planes_u64 = static_cast<size_t>(p - h->d_level_buf);
+  lb.planes_u64 = static_cast<size_t>(p - base);
   p += static_cast<size_t>(n_stats_nodes) * 3;
-  lb.chunk_u64 = static_cast<size_t>(p - h->d_level_buf);
+  lb.chunk_u64 = static_cast<size_t>(p - base);
   lb.total_u64 = lb.chunk_u64 * lb.W;
   return lb;
 }
@@ -395,7 +397,6 @@ int for_hist_kernel(bool hess, int mode, F f, bool multi = false) {
   }
   if (hess) return f(k_hist<true, kHistShared>);
   if (mode == kHistRootSum) return f(k_hist<false, kHistRootSum>);
-  if (mode == kHistPrivate) return f(k_hist<false, kHistPrivate>);
   if (mode == kHistPacked) return f(k_hist<false, kHistPacked>);
   return f(k_hist<false, kHistShared>);
 }
@@ -469,8 +470,6 @@ int configure_launches(ygg_gbt* h) {
     size_t max_smem = 0;
     for (int l = 0; l < h->num_levels; l++)
       if (h->hist_mode[l] == mode) max_smem = std::max(max_smem, h->hist_smem[l]);
-    // the debug seam runs the private layout on level-0 geometry
-    if (mode == kHistPrivate && !hh) max_smem = std::max(max_smem, hist_smem_bytes(1, 1, false, kHistPrivate));
     if (mode == kHistPacked && !hh) max_smem = std::max<size_t>(max_smem, 1);  // a level may fall back to / from it
     if (mode == kHistShared && !hh) max_smem = std::max<size_t>(max_smem, 1);
     if (max_smem == 0) continue;
@@ -559,9 +558,12 @@ int configure_launches(ygg_gbt* h) {
           it = max_of_chunk.emplace(chunk, m).first;
         }
         if (it->second <= kPackedMaxUpdates) break;
-        // shrink the chunk in proportion (+ margin); below one sub-chunk the flushes would cost more than the RED saves
+        // shrink the chunk in proportion (+ margin); below one sub-chunk the flushes would cost more than the RED saves.
+        // A proportional step that lands below one sub-chunk still tries the single sub-chunk before giving up (a bin
+        // that fills most of every block fits at one sub-chunk although two of them overflow).
         const int smaller = static_cast<int>(static_cast<double>(chunk) * 0.9 * kPackedMaxUpdates / it->second) / kSubBlocks * kSubBlocks;
-        chunk = std::min(smaller, chunk - kSubBlocks);
+        const int next = std::min(smaller, chunk - kSubBlocks);
+        chunk = (next < kSubBlocks && chunk > kSubBlocks) ? kSubBlocks : next;
       }
       if (chunk < kSubBlocks) {   // heavy bins (a dominant value / category): the carry-detecting layout, any chunk size
         h->hist_mode[l] = kHistShared;
@@ -632,8 +634,6 @@ int allocate_level_buffers(ygg_gbt* h) {
     const int stats_nodes = l == 0 ? 1 : (2 << (l - 1));
     max_u64 = std::max(max_u64, level_buf(h, slots, stats_nodes).total_u64);
   }
-  // debug seam: one slot over the hist features
-  max_u64 = std::max(max_u64, level_buf(h, 1, 1).total_u64);
   (void)f_hist;
   h->level_buf_bytes = max_u64 * sizeof(unsigned long long);
   YGG_RETURN_IF_ERROR(dev_alloc_plain(&h->d_level_buf, max_u64));
@@ -688,6 +688,69 @@ int ensure_root_counts(ygg_gbt* h) {
   YGG_RETURN_IF_ERROR(check_launch("k_root_counts"));
   h->root_cnt_valid = true;
   return YGG_OK;
+}
+
+// One level's histogram launch: what configure_launches chose for a level, or a plan of ygg_debug_level_histogram.
+struct HistLaunch {
+  int mode;            // k_hist layout; with k_hist2: kHistRootSum at the root, kHistPacked below
+  int G, S;            // features per work item, shared-memory slots (multi-pass: window + 1 dummy slot)
+  int chunk, grid;     // row blocks per work item, CTAs
+  int window, passes;  // window > 0: k_hist<., ., MULTI> over `passes` windows of `window` slots
+  int FL, T;           // FL > 0: k_hist2 with FL feature lanes and T sub-tiles per tile
+};
+HistLaunch level_launch(const ygg_gbt* h, int l) {
+  HistLaunch pl{};
+  pl.mode = h->hist_mode[l]; pl.G = h->hist_G[l]; pl.S = h->hist_S[l];
+  pl.chunk = h->hist_chunk[l]; pl.grid = h->hist_grid[l];
+  pl.passes = h->hist_passes[l]; pl.window = pl.passes > 1 ? pl.S - 1 : 0;
+  pl.FL = h->hist2_FL[l]; pl.T = h->hist2_T[l];
+  return pl;
+}
+
+// The histogram phase of level l: zeroes the planes of `lb` (not its stats tail), copies the precomputed root counts
+// (root layouts) and accumulates the level's active lists (d_act / d_act_h / d_q24 ...) into the slot histograms;
+// `levels[l]` gives the slots in use.  The level loop of grow_tree and ygg_debug_level_histogram both run it.
+int accumulate_level(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* levels, const HistLaunch& pl) {
+  const ygg_dataset* ds = h->ds;
+  const int hist_f_count = h->hist_f_end - h->hist_f_begin;
+  YGG_RETURN_IF_ERROR(zero_planes(h, lb));
+  if (pl.mode == kHistRootSum) {
+    // the root's counts do not depend on the gradients: reuse the precomputed (per-rank) ones,
+    // d_root_cnt is [W * f_chunk][256] so that every chunk's count plane is one row of a 2-D copy
+    const size_t row = static_cast<size_t>(lb.f_chunk) * kMaxBins * sizeof(uint32_t);
+    YGG_CUDA(cudaMemcpy2DAsync(lb.cnt, lb.chunk_u64 * sizeof(unsigned long long), h->d_root_cnt, row, row, lb.W,
+                               cudaMemcpyDeviceToDevice, h->stream));
+  }
+  if (pl.FL > 0) {
+    YGG_RETURN_IF_ERROR(ensure_bins4(h->ds));
+    Hist2Params hp{};
+    hp.bins4 = ds->d_bins4; hp.n_pad = ds->n_pad; hp.n = ds->n; hp.q24 = h->d_q24; hp.act = h->d_act;
+    hp.act_count = h->d_act_count; hp.act_sub = h->d_act_sub; hp.n_blocks = h->n_blocks;
+    hp.f_begin = h->hist_f_begin; hp.f_count = hist_f_count;
+    hp.g_begin = h->hist_f_begin / 4; hp.n_groups = (h->hist_f_end + 3) / 4 - hp.g_begin;
+    hp.S = pl.S; hp.T = pl.T; hp.chunk_blocks = pl.chunk;
+    hp.level = l; hp.levels = levels;
+    hp.hist_sum = lb.sum; hp.hist_cnt = lb.cnt;
+    hp.f_chunk = lb.f_chunk; hp.chunk_stride = static_cast<long long>(lb.chunk_u64);
+    return launch_hist2(h, hp, pl.FL, l == 0, pl.grid);
+  }
+  HistParams hp{};
+  hp.bins = ds->d_bins; hp.n_pad = ds->n_pad; hp.act = h->d_act; hp.act_h = h->d_act_h; hp.q24 = h->d_q24;
+  hp.act_count = h->d_act_count; hp.n_blocks = h->n_blocks;
+  hp.f_begin = h->hist_f_begin; hp.f_count = hist_f_count; hp.G = pl.G; hp.S = pl.S;
+  hp.chunk_blocks = pl.chunk;
+  hp.level = l; hp.levels = levels;
+  hp.hist_sum = lb.sum; hp.hist_cnt = lb.cnt; hp.hist_hsum = lb.hsum;
+  hp.f_chunk = lb.f_chunk; hp.chunk_stride = static_cast<long long>(lb.chunk_u64);
+  const size_t smem = hist_smem_bytes(pl.G, pl.S, hist_hess(h), pl.mode);
+  if (pl.window > 0) {
+    for (int pass = 0; pass < pl.passes; pass++) {
+      hp.level = l | ((pass * pl.window) << 8) | (pl.window << 20);   // slot window of this pass (HistParams.level)
+      YGG_RETURN_IF_ERROR(launch_hist(h, hp, pl.mode, pl.grid, smem, true));
+    }
+    return YGG_OK;
+  }
+  return launch_hist(h, hp, pl.mode, pl.grid, smem);
 }
 
 int elementwise_grid(const ygg_gbt* h) { return h->ds->num_sms * 8; }
@@ -795,46 +858,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
                                                 "hist_L12", "hist_L13", "hist_L14", "hist_L15"};
       ProfScope ps(h, "hist");
       ProfScope ps_level(h, kHistLevelNames[l & 15]);
-      // zero the histogram planes (not the stats tail, which holds this level's node statistics)
-      YGG_RETURN_IF_ERROR(zero_planes(h, lb));
-      if (h->hist_mode[l] == kHistRootSum) {
-        // the root's counts do not depend on the gradients: reuse the precomputed (per-rank) ones,
-        // d_root_cnt is [W * f_chunk][256] so that every chunk's count plane is one row of a 2-D copy
-        const size_t row = static_cast<size_t>(lb.f_chunk) * kMaxBins * sizeof(uint32_t);
-        YGG_CUDA(cudaMemcpy2DAsync(lb.cnt, lb.chunk_u64 * sizeof(unsigned long long), h->d_root_cnt, row, row, lb.W,
-                                   cudaMemcpyDeviceToDevice, h->stream));
-      }
-      if (h->hist2_FL[l] > 0) {
-        YGG_RETURN_IF_ERROR(ensure_bins4(h->ds));
-        Hist2Params hp{};
-        hp.bins4 = ds->d_bins4; hp.n_pad = ds->n_pad; hp.n = ds->n; hp.q24 = h->d_q24; hp.act = h->d_act;
-        hp.act_count = h->d_act_count; hp.act_sub = h->d_act_sub; hp.n_blocks = h->n_blocks;
-        hp.f_begin = h->hist_f_begin; hp.f_count = hist_f_count;
-        hp.g_begin = h->hist_f_begin / 4; hp.n_groups = (h->hist_f_end + 3) / 4 - hp.g_begin;
-        hp.S = h->hist_S[l]; hp.T = h->hist2_T[l]; hp.chunk_blocks = h->hist_chunk[l];
-        hp.level = l; hp.levels = h->d_levels;
-        hp.hist_sum = lb.sum; hp.hist_cnt = lb.cnt;
-        hp.f_chunk = lb.f_chunk; hp.chunk_stride = static_cast<long long>(lb.chunk_u64);
-        YGG_RETURN_IF_ERROR(launch_hist2(h, hp, h->hist2_FL[l], l == 0, h->hist_grid[l]));
-      } else {
-      HistParams hp{};
-      hp.bins = ds->d_bins; hp.n_pad = ds->n_pad; hp.act = h->d_act; hp.act_h = h->d_act_h; hp.q24 = h->d_q24;
-      hp.act_count = h->d_act_count; hp.n_blocks = h->n_blocks;
-      hp.f_begin = h->hist_f_begin; hp.f_count = hist_f_count; hp.G = h->hist_G[l]; hp.S = h->hist_S[l];
-      hp.chunk_blocks = h->hist_chunk[l];
-      hp.level = l; hp.levels = h->d_levels;
-      hp.hist_sum = lb.sum; hp.hist_cnt = lb.cnt; hp.hist_hsum = lb.hsum;
-      hp.f_chunk = lb.f_chunk; hp.chunk_stride = static_cast<long long>(lb.chunk_u64);
-      if (h->hist_passes[l] > 1) {
-        const int window = h->hist_S[l] - 1;
-        for (int pass = 0; pass < h->hist_passes[l]; pass++) {
-          hp.level = l | ((pass * window) << 8) | (window << 20);   // slot window of this pass (HistParams.level)
-          YGG_RETURN_IF_ERROR(launch_hist(h, hp, h->hist_mode[l], h->hist_grid[l], h->hist_smem[l], true));
-        }
-      } else {
-        YGG_RETURN_IF_ERROR(launch_hist(h, hp, h->hist_mode[l], h->hist_grid[l], h->hist_smem[l]));
-      }
-      }
+      YGG_RETURN_IF_ERROR(accumulate_level(h, l, lb, h->d_levels, level_launch(h, l)));
     }
     // after the collective this rank's statistics of the level sit in `level_stats`
     const unsigned long long* level_stats = lb.stats;
@@ -991,24 +1015,15 @@ __global__ void k_absmax(const float* g, int64_t n, DeviceState* st) {
   if ((threadIdx.x & 31) == 0) atomicMax(&st->gmax_bits, __float_as_uint(m));
 }
 
-// Debug seam: dense "active list" selecting the rows of one node (inactive rows get count 0 by
-// being routed to slot 0 with... no: they are simply left out block by block on the host side of the
-// list, so this kernel builds the list with a per-block serial compaction — test sizes only).
-__global__ void k_debug_actlists(const float* g, const int32_t* node_of_row, int node, int64_t n, int n_blocks,
-                                 const DeviceState* st, uint2* act, int32_t* act_count) {
-  const float P = pow2_cover(st->gmax_bits);
-  const float qscale = static_cast<float>(1u << (kQBits - 1)) / P;
-  for (int blk = blockIdx.x * blockDim.x + threadIdx.x; blk < n_blocks; blk += gridDim.x * blockDim.x) {
-    int cnt = 0;
+// Level-histogram seam: puts the slot of every entry of the compacted active lists into bits 24..31 of its word, as
+// k_partition writes them (q24 | slot << 24).
+__global__ void k_tag_slots(uint2* act, const int32_t* act_count, const uint8_t* slot_of_row, int n_blocks) {
+  for (int blk = blockIdx.x; blk < n_blocks; blk += gridDim.x) {
     const int64_t base = static_cast<int64_t>(blk) * kBlockRows;
-    for (int j = 0; j < kBlockRows; j++) {
-      const int64_t r = base + j;
-      if (r < n && node_of_row[r] == node) {
-        act[base + cnt] = make_uint2(quant_biased(g[r], qscale, kQBias, kQMax), static_cast<uint32_t>(j));
-        cnt++;
-      }
+    for (int i = threadIdx.x; i < act_count[blk]; i += blockDim.x) {
+      const uint2 e = act[base + i];
+      act[base + i] = make_uint2(e.x | (static_cast<uint32_t>(slot_of_row[base + e.y]) << 24), e.y);
     }
-    act_count[blk] = cnt;
   }
 }
 
@@ -2629,63 +2644,189 @@ int ygg_tree_train_on_gradients(ygg_gbt* h, const float* gradients, const float*
   return YGG_OK;
 }
 
-int ygg_debug_histogram(ygg_gbt* h, const float* gradients, const int32_t* node_of_row, int32_t node,
-                        int32_t feature, double* out_sum, int64_t* out_count) {
-  if (!h || !gradients || !node_of_row || !out_sum || !out_count) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
-  if (feature < h->hist_f_begin || feature >= h->hist_f_end) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d outside this shard", feature);
+int ygg_debug_hist_plan(const ygg_gbt* h, int32_t level, ygg_hist_plan* out) {
+  if (!h || !out) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (level < 0 || level >= h->num_levels) return set_error(YGG_ERR_INVALID_ARGUMENT, "level %d outside [0, %d)", level, h->num_levels);
+  ygg_hist_plan p{};
+  if (h->hist2_FL[level] > 0) {
+    p.mode = YGG_HIST_HIST2; p.group = h->hist2_FL[level]; p.hist2_tiles = h->hist2_T[level];
+  } else {
+    const int m = h->hist_mode[level];
+    p.mode = m == kHistRootSum ? YGG_HIST_ROOT_SUM : m == kHistPacked ? YGG_HIST_PACKED : YGG_HIST_SHARED;
+    p.group = h->hist_G[level];
+  }
+  p.chunk_blocks = h->hist_chunk[level];
+  p.slot_window = h->hist_passes[level] > 1 ? h->hist_S[level] - 1 : 0;
+  p.grid = h->hist_grid[level];
+  *out = p;
+  return YGG_OK;
+}
+
+int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* plan, const float* gradients,
+                              const float* second, const int32_t* slot_of_row, int32_t n_slots, uint64_t* out_sum,
+                              uint32_t* out_cnt, uint64_t* out_second, float* out_scales) {
+  if (!h || !gradients || !slot_of_row || !out_sum || !out_cnt || !out_scales) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (level < 0 || level >= h->num_levels) return set_error(YGG_ERR_INVALID_ARGUMENT, "level %d outside [0, %d)", level, h->num_levels);
+  if (n_slots < 1 || n_slots > 254) return set_error(YGG_ERR_INVALID_ARGUMENT, "n_slots=%d outside [1, 254] (8-bit slots)", n_slots);
+  const bool hh = hist_hess(h);
+  if (hh != (second != nullptr) || hh != (out_second != nullptr))
+    return set_error(YGG_ERR_INVALID_ARGUMENT, hh ? "this handle keeps a second histogram plane: `second` and `out_second` are required"
+                                                  : "this handle keeps no second histogram plane: `second` and `out_second` must be NULL");
+  // the power of two the second plane is quantised against (k_quantize's hqscale)
+  const float v_pow2 = hh ? (weighted(h) ? h->w_pow2 : h_pow2_of(h)) : 0.f;
+  const int64_t n = h->ds->n;
+  bool all_slot0 = true;
+  for (int64_t r = 0; r < n; r++) {
+    if (!std::isfinite(gradients[r])) return set_error(YGG_ERR_INVALID_ARGUMENT, "gradient of row %lld is not finite", static_cast<long long>(r));
+    if (hh && !(second[r] >= 0.f && second[r] <= v_pow2))
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "second-plane value of row %lld outside [0, %g]", static_cast<long long>(r), v_pow2);
+    if (slot_of_row[r] < -1 || slot_of_row[r] >= n_slots)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "slot %d of row %lld outside [-1, %d)", slot_of_row[r], static_cast<long long>(r), n_slots);
+    all_slot0 &= slot_of_row[r] == 0;
+  }
+  // the launch, validated on the host: a plan the kernels cannot run exactly is refused, never launched
+  HistLaunch pl{};
+  if (plan == nullptr) {
+    pl = level_launch(h, level);
+    if (n_slots > level_slot_bound(h, level))
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "the plan of level %d holds %d slots, %d requested", level, level_slot_bound(h, level), n_slots);
+  } else {
+    const ygg_hist_plan& p = *plan;
+    if (p.mode < YGG_HIST_ROOT_SUM || p.mode > YGG_HIST_HIST2) return set_error(YGG_ERR_INVALID_ARGUMENT, "unknown mode %d", p.mode);
+    if (p.chunk_blocks < 1 || p.chunk_blocks > kHistMaxChunkBlocks)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "chunk_blocks=%d outside [1, %d]", p.chunk_blocks, kHistMaxChunkBlocks);
+    if (p.grid < 1 || p.grid > 65535) return set_error(YGG_ERR_INVALID_ARGUMENT, "grid=%d outside [1, 65535]", p.grid);
+    if (p.slot_window < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "slot_window=%d", p.slot_window);
+    pl.chunk = p.chunk_blocks; pl.grid = p.grid;
+    if (p.mode == YGG_HIST_HIST2) {
+      if (p.group != 8 && p.group != 16 && p.group != 32) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2: %d feature lanes (8, 16 or 32)", p.group);
+      if (p.hist2_tiles != 1 && p.hist2_tiles != 2) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2: %d sub-tiles (1 or 2)", p.hist2_tiles);
+      if (p.slot_window != 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2 has no multi-pass form");
+      if (n_slots > 2) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2 with %d slots (at most 2)", n_slots);
+      if (hist2_smem_bytes(p.group, n_slots, p.hist2_tiles, level == 0) > 216 * 1024)
+        return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2 needs %zu bytes of shared memory (budget 216 KB)", hist2_smem_bytes(p.group, n_slots, p.hist2_tiles, level == 0));
+      pl.FL = p.group; pl.T = p.hist2_tiles; pl.S = n_slots; pl.G = 1; pl.passes = 1;
+      pl.mode = level == 0 ? kHistRootSum : kHistPacked;
+    } else {
+      if (p.group < 1 || p.group > 8) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist: group=%d outside [1, 8]", p.group);
+      pl.mode = p.mode == YGG_HIST_ROOT_SUM ? kHistRootSum : p.mode == YGG_HIST_PACKED ? kHistPacked : kHistShared;
+      pl.G = p.group;
+      if (p.slot_window > 0) {
+        if (pl.mode == kHistRootSum) return set_error(YGG_ERR_INVALID_ARGUMENT, "the root layout has no multi-pass form");
+        pl.window = p.slot_window; pl.S = p.slot_window + 1; pl.passes = (n_slots + p.slot_window - 1) / p.slot_window;
+      } else {
+        pl.S = n_slots; pl.passes = 1;
+      }
+      if (hist_smem_bytes(pl.G, pl.S, hh, pl.mode) > 224 * 1024)
+        return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist with G=%d and %d slots per pass needs %zu bytes of shared memory (budget 224 KB)",
+                         pl.G, pl.S, hist_smem_bytes(pl.G, pl.S, hh, pl.mode));
+    }
+  }
+  if (hh && (pl.FL > 0 || pl.mode != kHistShared))
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "a second histogram plane is accumulated by the shared layout only");
+  if (pl.mode == kHistRootSum && (level != 0 || sampling(h) || !all_slot0 || n_slots != 1))
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "the root layouts need level 0, no row sampling and every row in slot 0");
   YGG_CUDA(cudaSetDevice(h->ds->device));
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
-  YGG_RETURN_IF_ERROR(apply_pending(h));
-  const int64_t n = h->ds->n;
-  int32_t* d_nor = nullptr;
-  YGG_RETURN_IF_ERROR(dev_alloc(&d_nor, n));
-  YGG_CUDA(cudaMemcpyAsync(h->d_g, gradients, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  YGG_CUDA(cudaMemcpyAsync(d_nor, node_of_row, n * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
-  k_begin_iteration<<<1, 1, 0, h->stream>>>(h->d_st, h->d_levels, h->d_fam[0], h->d_slot_node[0], 1);
-  h->launches_total++;
-  k_absmax<<<elementwise_grid(h), 256, 0, h->stream>>>(h->d_g, n, h->d_st);
-  h->launches_total++;
-  k_debug_actlists<<<(h->n_blocks + 63) / 64, 64, 0, h->stream>>>(h->d_g, d_nor, node, n, h->n_blocks, h->d_st,
-                                                                   h->d_act, h->d_act_count);
-  h->launches_total++;
-  YGG_RETURN_IF_ERROR(check_launch("k_debug_actlists"));
-  const int f_count = h->hist_f_end - h->hist_f_begin;
-  const LevelBuf lb = level_buf(h, 1, 1);
-  YGG_RETURN_IF_ERROR(zero_planes(h, lb));
-  HistParams hp{};
-  hp.bins = h->ds->d_bins; hp.n_pad = h->ds->n_pad; hp.act = h->d_act; hp.act_h = h->d_act_h; hp.q24 = h->d_q24;
-  hp.act_count = h->d_act_count; hp.n_blocks = h->n_blocks;
-  hp.f_begin = h->hist_f_begin; hp.f_count = f_count; hp.G = 1; hp.S = 1;
-  hp.chunk_blocks = h->hist_chunk[0];
-  hp.level = 0; hp.levels = h->d_levels;
-  hp.hist_sum = lb.sum; hp.hist_cnt = lb.cnt; hp.hist_hsum = lb.hsum;
-  hp.f_chunk = lb.f_chunk; hp.chunk_stride = static_cast<long long>(lb.chunk_u64);
-  const int dbg_mode = hist_hess(h) ? kHistShared : kHistPrivate;
-  if (hist_hess(h)) YGG_CUDA(cudaMemsetAsync(h->d_act_h, 0, h->ds->n_pad * sizeof(uint32_t), h->stream));
-  YGG_RETURN_IF_ERROR(launch_hist(h, hp, dbg_mode, h->hist_grid[0], hist_smem_bytes(1, 1, hist_hess(h), dbg_mode)));
-  std::vector<unsigned long long> sum(kMaxBins);
-  std::vector<uint32_t> cnt(kMaxBins);
-  DeviceState st;
-  size_t off_cnt;
-  const size_t off = slot_hist_offset(0, feature - h->hist_f_begin, 0, lb.f_chunk, static_cast<long long>(lb.chunk_u64), &off_cnt);
-  YGG_CUDA(cudaMemcpyAsync(sum.data(), lb.sum + off, sizeof(unsigned long long) * kMaxBins, cudaMemcpyDeviceToHost, h->stream));
-  YGG_CUDA(cudaMemcpyAsync(cnt.data(), lb.cnt + off_cnt, sizeof(uint32_t) * kMaxBins, cudaMemcpyDeviceToHost, h->stream));
-  YGG_CUDA(cudaMemcpyAsync(&st, h->d_st, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
-  YGG_CUDA(cudaStreamSynchronize(h->stream));
-  dev_free(d_nor);
-  const float P = [&]() {
-    const unsigned bits = st.gmax_bits;
-    if (bits == 0u) return 1.f;
-    const int e = static_cast<int>(bits >> 23) - 127;
-    return (bits & 0x7FFFFFu) == 0u ? std::ldexp(1.f, e) : std::ldexp(1.f, e + 1);
-  }();
-  const double inv = static_cast<double>(P) / static_cast<double>(1u << (kQBits - 1));
-  const int B = h->ds->num_bins[feature];
-  for (int b = 0; b < B; b++) {
-    out_count[b] = cnt[b];
-    out_sum[b] = (static_cast<double>(static_cast<long long>(sum[b])) - static_cast<double>(cnt[b]) * static_cast<double>(kQBias)) * inv;
+  if (pl.mode == kHistPacked) {   // k_hist packed words, or k_hist2 below the root
+    const int sub = sub_blocks_of(h);
+    if (pl.chunk % sub != 0)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "packed layout: chunk_blocks=%d is not a multiple of the %d-block sub-chunk", pl.chunk, sub);
+    uint32_t* d_sub = nullptr;
+    uint32_t m = 0;
+    const int st = chunk_max_count(h, pl.chunk, &d_sub, &m);
+    dev_free(d_sub);
+    YGG_RETURN_IF_ERROR(st);
+    if (m > kPackedMaxUpdates)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "packed layout: a bin receives %u rows in one chunk of %d blocks (at most %u)", m, pl.chunk, kPackedMaxUpdates);
   }
-  return YGG_OK;
+  if (pl.mode == kHistRootSum) YGG_RETURN_IF_ERROR(ensure_root_counts(h));
+  if (pl.FL == 0) {   // the per-kernel shared-memory cap (configure_launches raises it only for the layouts the handle runs)
+    const int st = for_hist_kernel(hh, pl.mode, [&](auto kern) -> int {
+      YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+      return YGG_OK;
+    }, pl.window > 0);
+    if (st != YGG_OK) return st;
+  }
+
+  // Inputs in the training format.  Temporaries for everything the boosting state keeps (gradients, node ids, device
+  // scalars, level descriptors, level buffer); the active lists, q24 / hq24 and act_sub are scratch every iteration rewrites.
+  const int64_t n_pad = h->ds->n_pad;
+  const int f_hist = h->hist_f_end - h->hist_f_begin;
+  std::vector<uint8_t> sel(n), slot8(n);
+  for (int64_t r = 0; r < n; r++) {
+    sel[r] = slot_of_row[r] >= 0 ? 1 : 0;
+    slot8[r] = static_cast<uint8_t>(slot_of_row[r] >= 0 ? slot_of_row[r] : 0);
+  }
+  std::vector<LevelDesc> lv(32, LevelDesc{0, 0, 0, 0});
+  lv[level] = LevelDesc{0, n_slots, n_slots, 0};
+  const LevelBuf probe = level_buf(h, n_slots, 1);
+  float *d_g = nullptr, *d_v = nullptr;
+  uint8_t *d_sel = nullptr, *d_slot = nullptr;
+  uint16_t* d_nor = nullptr;
+  DeviceState* d_st = nullptr;
+  LevelDesc* d_lv = nullptr;
+  unsigned long long *d_stats = nullptr, *d_buf = nullptr;
+  auto run = [&]() -> int {
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_g, n));
+    if (hh) YGG_RETURN_IF_ERROR(dev_alloc(&d_v, n));
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_sel, n));
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_slot, n));
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_nor, n_pad));
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_st, 1));
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_lv, lv.size()));
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_stats, 3));
+    YGG_RETURN_IF_ERROR(dev_alloc(&d_buf, probe.total_u64));
+    YGG_CUDA(cudaMemcpyAsync(d_g, gradients, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    if (hh) YGG_CUDA(cudaMemcpyAsync(d_v, second, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    YGG_CUDA(cudaMemcpyAsync(d_sel, sel.data(), n, cudaMemcpyHostToDevice, h->stream));
+    YGG_CUDA(cudaMemcpyAsync(d_slot, slot8.data(), n, cudaMemcpyHostToDevice, h->stream));
+    YGG_CUDA(cudaMemcpyAsync(d_lv, lv.data(), lv.size() * sizeof(LevelDesc), cudaMemcpyHostToDevice, h->stream));
+    k_absmax<<<elementwise_grid(h), 256, 0, h->stream>>>(d_g, n, d_st);
+    QuantParams q{};
+    q.n = n; q.n_pad = n_pad; q.g = d_g; q.h = d_v;
+    q.q24 = h->d_q24; q.hq24 = hh ? h->d_hq24 : nullptr;
+    q.act = h->d_act; q.act_h = h->d_act_h; q.act_count = h->d_act_count;
+    q.node_of_row = d_nor; q.st = d_st; q.stats = d_stats; q.root_candidate = 1;
+    q.h_pow2 = hh ? v_pow2 : 1.f;
+    k_quantize<<<elementwise_grid(h), 256, 0, h->stream>>>(q);
+    YGG_RETURN_IF_ERROR(check_launch("k_quantize"));
+    // the rows of the slots, in row order, with their slots: the lists k_partition writes
+    const int cgrid = std::min(h->n_blocks, h->ds->num_sms * 4);
+    k_compact_root<<<cgrid, kCompactThreads, 0, h->stream>>>(h->d_act, hh ? h->d_act_h : nullptr, h->d_act_count, h->d_act_sub, d_sel, n,
+                                                             h->n_blocks);
+    YGG_RETURN_IF_ERROR(check_launch("k_compact_root"));
+    k_tag_slots<<<cgrid, 256, 0, h->stream>>>(h->d_act, h->d_act_count, d_slot, h->n_blocks);
+    YGG_RETURN_IF_ERROR(check_launch("k_tag_slots"));
+    h->launches_total += 4;
+    const LevelBuf lb = level_buf(h, n_slots, 1, d_buf);
+    YGG_RETURN_IF_ERROR(accumulate_level(h, level, lb, d_lv, pl));
+    std::vector<unsigned long long> buf(lb.total_u64);
+    DeviceState st;
+    YGG_CUDA(cudaMemcpyAsync(buf.data(), d_buf, lb.total_u64 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    YGG_CUDA(cudaMemcpyAsync(&st, d_st, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    YGG_CUDA(cudaStreamSynchronize(h->stream));
+    // de-chunk: [n_slots][f_hist][256]
+    const uint32_t* cnt = reinterpret_cast<const uint32_t*>(buf.data() + (reinterpret_cast<unsigned long long*>(lb.cnt) - d_buf));
+    for (int s = 0; s < n_slots; s++)
+      for (int f = 0; f < f_hist; f++)
+        for (int b = 0; b < kMaxBins; b++) {
+          size_t oc;
+          const size_t o = slot_hist_offset(s, f, b, lb.f_chunk, static_cast<long long>(lb.chunk_u64), &oc);
+          const size_t i = (static_cast<size_t>(s) * f_hist + f) * kMaxBins + b;
+          out_sum[i] = buf[o];
+          out_cnt[i] = cnt[oc];
+          if (hh) out_second[i] = buf[(lb.hsum - d_buf) + o];
+        }
+    out_scales[0] = st.g_pow2;
+    out_scales[1] = v_pow2;
+    return YGG_OK;
+  };
+  const int status = run();
+  cudaStreamSynchronize(h->stream);
+  dev_free(d_g); dev_free(d_v); dev_free(d_sel); dev_free(d_slot); dev_free(d_nor); dev_free(d_st); dev_free(d_lv);
+  dev_free(d_stats); dev_free(d_buf);
+  return status;
 }
 
 int ygg_partition_rows(ygg_dataset* ds, const uint32_t* rows_in, int64_t n, int32_t feature,
