@@ -401,6 +401,17 @@ int for_hist_kernel(bool hess, int mode, F f, bool multi = false) {
   return f(k_hist<false, kHistShared>);
 }
 
+// Dynamic shared memory a k_hist CTA may use: the device's opt-in limit per block less the kernel's static shared
+// memory (s_counts; the same in every instantiation).
+int hist_smem_budget(int device, size_t* budget) {
+  int optin = 0;
+  YGG_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+  cudaFuncAttributes fa{};
+  YGG_CUDA(cudaFuncGetAttributes(&fa, k_hist<false, kHistPacked>));
+  *budget = static_cast<size_t>(optin) - fa.sharedSizeBytes;
+  return YGG_OK;
+}
+
 // Largest per-bin row count of any (chunk of `chunk_blocks` blocks, histogrammed feature) of this handle's rows;
 // `*d_sub` caches the sub-chunk count table between calls (the caller frees it).
 // granularity of the packed-bound table and of the chunk sizes it allows: single blocks up to 4M rows (the chunk size is
@@ -428,7 +439,8 @@ int chunk_max_count(ygg_gbt* h, int chunk_blocks, uint32_t** d_sub, uint32_t* ou
 
 int configure_launches(ygg_gbt* h) {
   const bool hh = hist_hess(h);
-  const size_t budget = 224 * 1024;  // dynamic shared memory per CTA we are willing to use (227 KB max)
+  size_t budget = 0;
+  YGG_RETURN_IF_ERROR(hist_smem_budget(h->ds->device, &budget));
   const int f_count = h->hist_f_end - h->hist_f_begin;  // features histogrammed by this rank
   for (int l = 0; l < h->num_levels; l++) {
     // Lane-private (bank-conflict-free) layouts while they fit; the root additionally skips the
@@ -2717,9 +2729,11 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
       } else {
         pl.S = n_slots; pl.passes = 1;
       }
-      if (hist_smem_bytes(pl.G, pl.S, hh, pl.mode) > 224 * 1024)
-        return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist with G=%d and %d slots per pass needs %zu bytes of shared memory (budget 224 KB)",
-                         pl.G, pl.S, hist_smem_bytes(pl.G, pl.S, hh, pl.mode));
+      size_t budget = 0;
+      YGG_RETURN_IF_ERROR(hist_smem_budget(h->ds->device, &budget));
+      if (hist_smem_bytes(pl.G, pl.S, hh, pl.mode) > budget)
+        return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist with G=%d and %d slots per pass needs %zu bytes of shared memory (budget %zu)",
+                         pl.G, pl.S, hist_smem_bytes(pl.G, pl.S, hh, pl.mode), budget);
     }
   }
   if (hh && (pl.FL > 0 || pl.mode != kHistShared))
@@ -2742,8 +2756,10 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
   }
   if (pl.mode == kHistRootSum) YGG_RETURN_IF_ERROR(ensure_root_counts(h));
   if (pl.FL == 0) {   // the per-kernel shared-memory cap (configure_launches raises it only for the layouts the handle runs)
+    size_t budget = 0;
+    YGG_RETURN_IF_ERROR(hist_smem_budget(h->ds->device, &budget));
     const int st = for_hist_kernel(hh, pl.mode, [&](auto kern) -> int {
-      YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+      YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(budget)));
       return YGG_OK;
     }, pl.window > 0);
     if (st != YGG_OK) return st;

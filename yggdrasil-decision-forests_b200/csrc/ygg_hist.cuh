@@ -27,6 +27,7 @@
 // bandwidth — is what bounds this kernel (tools/atoms_bench.cu).
 #pragma once
 #include <cstdint>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 #include "ygg_device.cuh"
@@ -428,6 +429,36 @@ __global__ void __launch_bounds__(kHistThreads, 1) k_hist(HistParams p) {
                 }
                 }
               }
+            } else if constexpr (MODE == kHistPacked) {
+              // Tail of the block's active list.  A u slot covers 32 consecutive entries of the warp, so only the slot
+              // that holds the list's end is partly valid, and only in one warp per block: the slots holding entries run
+              // the unpredicated loop (the deep levels have 2-3 of them per block and warp, no slot full in every lane),
+              // the invalid lanes of the partial one add zero (their entries were loaded as 0: bin 0 of slot 0).
+              const int nv = min(kHistUnroll, (n_act - wb + kHistThreads - 1) / kHistThreads);   // >= 1, warp-uniform
+              auto packed_tail = [&](auto nv_c) {
+                constexpr int NV = decltype(nv_c)::value;
+                uint32_t inc[NV];
+#pragma unroll
+                for (int u = 0; u < NV; u++)
+                  inc[u] = ok[u] ? ((((cur[u].x >> kPackedCoarseShift) & 0x3Fu) << kPackedCntBits) | 1u) : 0u;
+                for (int gi = 0; gi < gcount; gi++) {
+                  const uint32_t fbase = s_hist + static_cast<uint32_t>(gi * bins_per_feature) * 4u;
+                  const uint32_t tbase = tile + gi * kBlockRows;
+                  uint32_t addr[NV];
+#pragma unroll
+                  for (int u = 0; u < NV; u++) addr[u] = fbase + bin_offset(cur[u].x, smem_ld_u8(tbase + cur[u].y));
+#pragma unroll
+                  for (int u = 0; u < NV; u++) {
+                    smem_red(addr[u], inc[u]);
+                    smem_red(addr[u] + plane_bytes, cur[u].x & kQMax);
+                  }
+                }
+              };
+              static_assert(kHistUnroll == 4, "packed_tail dispatch");
+              if (nv == 1) packed_tail(std::integral_constant<int, 1>{});
+              else if (nv == 2) packed_tail(std::integral_constant<int, 2>{});
+              else if (nv == 3) packed_tail(std::integral_constant<int, 3>{});
+              else packed_tail(std::integral_constant<int, 4>{});
             } else {
               // tail of the block's active list
               for (int gi = 0; gi < gcount; gi++) {
