@@ -270,7 +270,7 @@ def test_reference_label_classes_order(label_data):
 def test_feature_lane_histogram_kernel_is_bit_identical(monkeypatch):
     """k_hist2 (csrc/ygg_hist2.cuh: lanes = features, [bin][feature] histograms, interleaved copy of the matrix) is an
     alternative to k_hist on the levels with <= 2 slots; integer sums make the two bit-identical.  Off by default
-    (it is not faster, DESIGN.md §5); YGG_HIST2=1 turns it on for handles created afterwards."""
+    (faster at the root only, DESIGN.md §5); YGG_HIST2=1 turns it on for handles created afterwards."""
     bins, nb, na, y = synth(60000, 40, seed=11, bins=255)
 
     def run():

@@ -121,6 +121,15 @@ struct LossRec {
 
 enum ShardMode { kShardNone = 0, kShardFeatures = 1, kShardRows = 2 };
 
+// One level's histogram launch: what configure_launches chose for a level, or a plan of ygg_debug_level_histogram.
+struct HistLaunch {
+  int mode;            // k_hist layout; with k_hist2: kHistRootSum at the root, kHistPacked below
+  int G, S;            // features per work item, shared-memory slots (multi-pass: window + 1 dummy slot)
+  int chunk, grid;     // row blocks per work item, CTAs
+  int window, passes;  // window > 0: k_hist<., ., MULTI> over `passes` windows of `window` slots
+  int FL, T;           // FL > 0: k_hist2 with FL feature lanes and T sub-tiles per tile
+};
+
 struct ygg_gbt {
   ygg_dataset* ds = nullptr;
   ygg_gbt_config cfg{};
@@ -229,10 +238,7 @@ struct ygg_gbt {
   void** d_peer_windows = nullptr;   // [world] best-split windows of every rank as mapped in this process (or null)
   uint32_t exchange_epoch = 0;
   // launch configuration
-  int hist_grid[32]{}, hist_G[32]{}, hist_S[32]{}, hist_chunk[32]{}, hist_mode[32]{};
-  int hist_passes[32]{};               // > 1: the level's slots are accumulated in windows of hist_S[l] - 1 slots (k_hist<.., MULTI>)
-  int hist2_FL[32]{}, hist2_T[32]{};   // > 0: the level runs k_hist2 with FL feature lanes and T sub-tiles per tile
-  size_t hist_smem[32]{};
+  HistLaunch hist_plan[32]{};   // per tree level
   int part_smem_children = 0;
   // profiling
   bool profiling = false;
@@ -411,6 +417,8 @@ int hist_smem_budget(int device, size_t* budget) {
   *budget = static_cast<size_t>(optin) - fa.sharedSizeBytes;
   return YGG_OK;
 }
+// Dynamic shared memory a k_hist2 CTA may use (it also holds 4.6 KB of static shared memory: the sub-tile offsets).
+constexpr size_t kHist2SmemBudget = 216 * 1024;
 
 // Largest per-bin row count of any (chunk of `chunk_blocks` blocks, histogrammed feature) of this handle's rows;
 // `*d_sub` caches the sub-chunk count table between calls (the caller frees it).
@@ -437,76 +445,50 @@ int chunk_max_count(ygg_gbt* h, int chunk_blocks, uint32_t** d_sub, uint32_t* ou
   return YGG_OK;
 }
 
+// Raises the dynamic shared-memory cap of every histogram kernel to its budget, once per device: the seven k_hist
+// instantiations for_hist_kernel returns and the six of k_hist2.  The cap only allows a launch to request that much
+// (every launch passes its exact size); it is per kernel and shared by every handle of the process (several handles
+// with different feature shards may coexist), hence always the full budget.
+int raise_hist_smem_caps_once(int device) {
+  static std::mutex mu;
+  static std::vector<char> done;
+  std::lock_guard<std::mutex> lock(mu);
+  if (static_cast<int>(done.size()) <= device) done.resize(device + 1, 0);
+  if (done[device]) return YGG_OK;
+  size_t budget = 0;
+  YGG_RETURN_IF_ERROR(hist_smem_budget(device, &budget));
+  auto set_cap = [](size_t bytes) {
+    return [bytes](auto kern) -> int {
+      YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
+      return YGG_OK;
+    };
+  };
+  for (const bool hess : {false, true})
+    for (const int mode : {kHistRootSum, kHistPacked, kHistShared})
+      for (const bool multi : {false, true}) YGG_RETURN_IF_ERROR(for_hist_kernel(hess, mode, set_cap(budget), multi));
+  const auto cap2 = set_cap(kHist2SmemBudget);
+  YGG_RETURN_IF_ERROR(cap2(k_hist2<32, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<32, false>));
+  YGG_RETURN_IF_ERROR(cap2(k_hist2<16, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<16, false>));
+  YGG_RETURN_IF_ERROR(cap2(k_hist2<8, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<8, false>));
+  done[device] = 1;
+  return YGG_OK;
+}
+
 int configure_launches(ygg_gbt* h) {
+  (void)cudaGetLastError();  // stale foreign error (see ygg_gbt_step): chunk_max_count's launch check would report it
   const bool hh = hist_hess(h);
   size_t budget = 0;
   YGG_RETURN_IF_ERROR(hist_smem_budget(h->ds->device, &budget));
+  YGG_RETURN_IF_ERROR(raise_hist_smem_caps_once(h->ds->device));
   const int f_count = h->hist_f_end - h->hist_f_begin;  // features histogrammed by this rank
-  for (int l = 0; l < h->num_levels; l++) {
-    // Lane-private (bank-conflict-free) layouts while they fit; the root additionally skips the
-    // count atomics (precomputed counts).
-    // The root skips the count atomics (its counts are gradient independent and precomputed).
-    // YGG_HIST_ROOT_SUM=0 disables that (tuning / A-B knob).
-    int mode = kHistShared;
-    if (!hh && l == 0 && !sampling(h)) {   // (a sampled root is not the whole dataset: its counts are not the precomputed ones)
-      const char* env = std::getenv("YGG_HIST_ROOT_SUM");
-      if (!env || std::atoi(env) != 0) mode = kHistRootSum;
-    }
-    if (!hh && (l > 0 || sampling(h))) {
-      // two REDs per element instead of RED + returning ATOMS; confirmed (or taken back) below, once the chunk
-      // sizes are known: no bin may receive more than 8191 updates inside one work item.  YGG_HIST_PACKED=0: A/B knob.
-      const char* env = std::getenv("YGG_HIST_PACKED");
-      if (!env || std::atoi(env) != 0) mode = kHistPacked;
-    }
-    int S = level_slot_bound(h, l);
-    h->hist_passes[l] = 1;
-    if (hist_smem_bytes(1, S, hh, mode) > budget) {
-      // more slots than shared memory holds: windows of S_pass slots (+ 1 dummy slot for the rows of the other windows),
-      // one launch per window.  The slot of a row travels in 8 bits of its active-list entry (0xFF = none).
-      if (S > 254)
-        return set_error(YGG_ERR_UNIMPLEMENTED, "max_depth=%d needs %d histogram slots at level %d; the active lists carry 8-bit slots",
-                         h->cfg.max_depth, S, l);
-      int s_pass = 1;
-      while (hist_smem_bytes(1, 2 * s_pass + 1, hh, mode) <= budget) s_pass *= 2;
-      h->hist_passes[l] = (S + s_pass - 1) / s_pass;
-      S = s_pass + 1;
-    }
-    int G = 1;
-    while (G < 8 && G < f_count && hist_smem_bytes(G + 1, S, hh, mode) <= budget) G++;
-    h->hist_G[l] = G;
-    h->hist_S[l] = S;
-    h->hist_mode[l] = mode;
-    h->hist_smem[l] = hist_smem_bytes(G, S, hh, mode);
-  }
-  for (int mode = 0; mode < 4; mode++) {
-    size_t max_smem = 0;
-    for (int l = 0; l < h->num_levels; l++)
-      if (h->hist_mode[l] == mode) max_smem = std::max(max_smem, h->hist_smem[l]);
-    if (mode == kHistPacked && !hh) max_smem = std::max<size_t>(max_smem, 1);  // a level may fall back to / from it
-    if (mode == kHistShared && !hh) max_smem = std::max<size_t>(max_smem, 1);
-    if (max_smem == 0) continue;
-    // The attribute is a per-kernel cap shared by every handle of the process (several handles with
-    // different feature shards may coexist): always raise it to the full budget.
-    const int st = for_hist_kernel(hh, mode, [&](auto kern) -> int {
-      YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(budget)));
-      return YGG_OK;
-    });
-    if (st != YGG_OK) return st;
-    if (hh) break;
-  }
   const int n_blocks = static_cast<int>(h->ds->n_pad / kBlockRows);
   const int kSubBlocks = sub_blocks_of(h);
-  static const double min_items = [] {   // tuning knob (default 3 work items per CTA)
-    const char* v = std::getenv("YGG_HIST_ITEMS_PER_CTA");
-    return v ? std::atof(v) : 1.0;   // measured: whole waves beat many small items on C2, C3 and at 1.25M rows per rank
-  }();
+  // Work items per CTA.  k_hist: measured, whole waves beat many small items on C2, C3 and at 1.25M rows per rank;
+  // k_hist2: few, equal items (one wave).
+  const double min_items = 1.0, min_items2 = 0.9;
   // Row blocks per work item (a multiple of `step`): as many as the bin counters allow (the flush to the global
   // histogram is amortised over the chunk), but few enough that every CTA gets >= min_items items, and among those
   // the size whose item count fills whole waves of the persistent grid (static round-robin over CTAs).
-  static const double min_items2 = [] {   // k_hist2 levels: few, equal items (default: one wave)
-    const char* v = std::getenv("YGG_HIST2_ITEMS_PER_CTA");
-    return v ? std::atof(v) : 0.9;
-  }();
   auto choose_chunk = [&](int n_fgroups, int grid, int step, double need) {
     const int max_c = std::max(step, kHistMaxChunkBlocks / step * step);
     const int min_chunks = std::max(1, (n_blocks + max_c - 1) / max_c);
@@ -528,29 +510,51 @@ int configure_launches(ygg_gbt* h) {
     return best;
   };
   // k_hist2 (feature-per-lane, bank-conflict-free; ygg_hist2.cuh) on the shallow levels.  OFF by default: measured on
-  // C3 it ties k_hist at the root and at level 1 and loses at level 2 (DESIGN.md §5),
-  // while costing a second copy of the matrix.  YGG_HIST2=1 enables it (read at every configure: tests toggle it).
+  // C3 it is faster than k_hist at the root but slower at levels 1 and 2 (DESIGN.md §5), while costing a second copy of
+  // the matrix.  YGG_HIST2=1 enables it (read at every configure: tests toggle it).
   const int g_begin = h->hist_f_begin / 4, n_groups = (h->hist_f_end + 3) / 4 - g_begin;
-  const size_t budget2 = 216 * 1024;   // k_hist2 also holds 4.6 KB of static shared memory (sub-tile offsets)
   const char* env_hist2 = std::getenv("YGG_HIST2");
   const bool want_hist2 = env_hist2 != nullptr && std::atoi(env_hist2) != 0;
   for (int l = 0; l < h->num_levels; l++) {
-    h->hist_grid[l] = h->ds->num_sms;  // persistent: one CTA per SM
-    h->hist2_FL[l] = 0;
-    const int S = h->hist_S[l];
+    HistLaunch& pl = h->hist_plan[l];
+    // The root skips the count atomics: its counts are gradient independent and precomputed (a sampled root is not the
+    // whole dataset: its counts are not the precomputed ones).  Below it, packed words: two REDs per element instead of
+    // RED + returning ATOMS; confirmed (or taken back) below, once the chunk sizes are known: no bin may receive more
+    // than 8191 updates inside one work item.
+    pl.mode = hh ? kHistShared : (l == 0 && !sampling(h)) ? kHistRootSum : kHistPacked;
+    int S = level_slot_bound(h, l);
+    pl.window = 0;
+    pl.passes = 1;
+    if (hist_smem_bytes(1, S, hh, pl.mode) > budget) {
+      // more slots than shared memory holds: windows of S_pass slots (+ 1 dummy slot for the rows of the other windows),
+      // one launch per window.  The slot of a row travels in 8 bits of its active-list entry (0xFF = none).
+      if (S > 254)
+        return set_error(YGG_ERR_UNIMPLEMENTED, "max_depth=%d needs %d histogram slots at level %d; the active lists carry 8-bit slots",
+                         h->cfg.max_depth, S, l);
+      int s_pass = 1;
+      while (hist_smem_bytes(1, 2 * s_pass + 1, hh, pl.mode) <= budget) s_pass *= 2;
+      pl.window = s_pass;
+      pl.passes = (S + s_pass - 1) / s_pass;
+      S = s_pass + 1;
+    }
+    int G = 1;
+    while (G < 8 && G < f_count && hist_smem_bytes(G + 1, S, hh, pl.mode) <= budget) G++;
+    pl.G = G;
+    pl.S = S;
+    pl.grid = h->ds->num_sms;  // persistent: one CTA per SM
+    pl.FL = pl.T = 0;
     // S <= 2: 32 feature lanes fit; at S = 4 only 16 would (two rows per instruction: bank conflicts come back and the
     // gain over k_hist is gone: tools/hist_loop_bench.cu)
-    if (want_hist2 && !hh && S <= 2 && (l > 0 || h->hist_mode[0] == kHistRootSum)) {
+    if (want_hist2 && !hh && S <= 2 && (l > 0 || pl.mode == kHistRootSum)) {
       int FL = 32;
       while (FL > 8 && FL / 2 >= 4 * n_groups) FL /= 2;   // few features: no idle lanes
       int T = 2;
-      if (hist2_smem_bytes(FL, S, T, l == 0) > budget2) T = 1;
-      if (hist2_smem_bytes(FL, S, T, l == 0) <= budget2) { h->hist2_FL[l] = FL; h->hist2_T[l] = T; }
+      if (hist2_smem_bytes(FL, S, T, l == 0) > kHist2SmemBudget) T = 1;
+      if (hist2_smem_bytes(FL, S, T, l == 0) <= kHist2SmemBudget) { pl.FL = FL; pl.T = T; }
     }
-    const bool packed = h->hist_mode[l] == kHistPacked || (h->hist2_FL[l] > 0 && l > 0);   // (k_hist2 is not used at a sampled root: hist_mode[0] != kHistRootSum)
-    const int n_fgroups = h->hist2_FL[l] > 0 ? (n_groups + h->hist2_FL[l] / 4 - 1) / (h->hist2_FL[l] / 4)
-                                              : (f_count + h->hist_G[l] - 1) / h->hist_G[l];
-    h->hist_chunk[l] = choose_chunk(n_fgroups, h->hist_grid[l], packed ? kSubBlocks : 1, h->hist2_FL[l] > 0 ? min_items2 : min_items);
+    const bool packed = pl.mode == kHistPacked || (pl.FL > 0 && l > 0);   // (k_hist2 is not used at a sampled root: its mode is not kHistRootSum)
+    const int n_fgroups = pl.FL > 0 ? (n_groups + pl.FL / 4 - 1) / (pl.FL / 4) : (f_count + G - 1) / G;
+    pl.chunk = choose_chunk(n_fgroups, pl.grid, packed ? kSubBlocks : 1, pl.FL > 0 ? min_items2 : min_items);
   }
   // Packed words (kHistPacked and k_hist2 below the root): the dataset-level bound on the updates a bin can receive
   // inside one work item (ygg_hist.cuh).
@@ -559,8 +563,9 @@ int configure_launches(ygg_gbt* h) {
     uint32_t* d_sub = nullptr;
     int status = YGG_OK;
     for (int l = 0; l < h->num_levels && status == YGG_OK; l++) {
-      if (h->hist_mode[l] != kHistPacked && (h->hist2_FL[l] == 0 || l == 0)) continue;
-      int chunk = h->hist_chunk[l];
+      HistLaunch& pl = h->hist_plan[l];
+      if (pl.mode != kHistPacked && (pl.FL == 0 || l == 0)) continue;
+      int chunk = pl.chunk;
       while (chunk >= kSubBlocks) {
         auto it = max_of_chunk.find(chunk);
         if (it == max_of_chunk.end()) {
@@ -578,40 +583,15 @@ int configure_launches(ygg_gbt* h) {
         chunk = (next < kSubBlocks && chunk > kSubBlocks) ? kSubBlocks : next;
       }
       if (chunk < kSubBlocks) {   // heavy bins (a dominant value / category): the carry-detecting layout, any chunk size
-        h->hist_mode[l] = kHistShared;
-        h->hist2_FL[l] = 0;
-        h->hist_chunk[l] = choose_chunk((f_count + h->hist_G[l] - 1) / h->hist_G[l], h->hist_grid[l], 1, min_items);
+        pl.mode = kHistShared;
+        pl.FL = 0;
+        pl.chunk = choose_chunk((f_count + pl.G - 1) / pl.G, pl.grid, 1, min_items);
       } else {
-        h->hist_chunk[l] = chunk;
+        pl.chunk = chunk;
       }
     }
     dev_free(d_sub);
     if (status != YGG_OK) return status;
-  }
-  {
-    auto set_attr = [&](auto kern) -> int {
-      YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(budget2)));
-      return YGG_OK;
-    };
-    bool any_multi = false;
-    for (int l = 0; l < h->num_levels; l++) any_multi |= h->hist_passes[l] > 1;
-    if (any_multi) {
-      const int st = for_hist_kernel(hh, kHistPacked, [&](auto kern) -> int {
-        YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(budget)));
-        return YGG_OK;
-      }, true);
-      if (st != YGG_OK) return st;
-      if (!hh) {
-        const int st2 = for_hist_kernel(false, kHistShared, [&](auto kern) -> int {
-          YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(budget)));
-          return YGG_OK;
-        }, true);
-        if (st2 != YGG_OK) return st2;
-      }
-    }
-    YGG_RETURN_IF_ERROR(set_attr(k_hist2<32, true>)); YGG_RETURN_IF_ERROR(set_attr(k_hist2<32, false>));
-    YGG_RETURN_IF_ERROR(set_attr(k_hist2<16, true>)); YGG_RETURN_IF_ERROR(set_attr(k_hist2<16, false>));
-    YGG_RETURN_IF_ERROR(set_attr(k_hist2<8, true>)); YGG_RETURN_IF_ERROR(set_attr(k_hist2<8, false>));
   }
   // k_partition shared accumulators: up to 32 KB (one copy) / 14 KB (lane-private, <= 16 children).
   h->part_smem_children = static_cast<int>((32 * 1024) / (kPartWords * sizeof(uint32_t)));
@@ -702,23 +682,6 @@ int ensure_root_counts(ygg_gbt* h) {
   return YGG_OK;
 }
 
-// One level's histogram launch: what configure_launches chose for a level, or a plan of ygg_debug_level_histogram.
-struct HistLaunch {
-  int mode;            // k_hist layout; with k_hist2: kHistRootSum at the root, kHistPacked below
-  int G, S;            // features per work item, shared-memory slots (multi-pass: window + 1 dummy slot)
-  int chunk, grid;     // row blocks per work item, CTAs
-  int window, passes;  // window > 0: k_hist<., ., MULTI> over `passes` windows of `window` slots
-  int FL, T;           // FL > 0: k_hist2 with FL feature lanes and T sub-tiles per tile
-};
-HistLaunch level_launch(const ygg_gbt* h, int l) {
-  HistLaunch pl{};
-  pl.mode = h->hist_mode[l]; pl.G = h->hist_G[l]; pl.S = h->hist_S[l];
-  pl.chunk = h->hist_chunk[l]; pl.grid = h->hist_grid[l];
-  pl.passes = h->hist_passes[l]; pl.window = pl.passes > 1 ? pl.S - 1 : 0;
-  pl.FL = h->hist2_FL[l]; pl.T = h->hist2_T[l];
-  return pl;
-}
-
 // The histogram phase of level l: zeroes the planes of `lb` (not its stats tail), copies the precomputed root counts
 // (root layouts) and accumulates the level's active lists (d_act / d_act_h / d_q24 ...) into the slot histograms;
 // `levels[l]` gives the slots in use.  The level loop of grow_tree and ygg_debug_level_histogram both run it.
@@ -806,7 +769,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
   const bool rows_sharded = h->shard_mode == kShardRows;
   const int64_t n_job = sampling(h) ? h->n_selected : (rows_sharded ? h->n_global : ds->n);   // rows the tree is trained on
   const int root_candidate = (n_job >= h->cfg.min_examples && 1 < h->cfg.max_depth) ? 1 : 0;
-  if (h->num_levels > 0 && h->hist_mode[0] == kHistRootSum) YGG_RETURN_IF_ERROR(ensure_root_counts(h));
+  if (h->num_levels > 0 && h->hist_plan[0].mode == kHistRootSum) YGG_RETURN_IF_ERROR(ensure_root_counts(h));
   const bool hess = hist_hess(h);
   auto slots_of = [&](int l) { return level_slot_bound(h, l); };
   {
@@ -870,7 +833,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
                                                 "hist_L12", "hist_L13", "hist_L14", "hist_L15"};
       ProfScope ps(h, "hist");
       ProfScope ps_level(h, kHistLevelNames[l & 15]);
-      YGG_RETURN_IF_ERROR(accumulate_level(h, l, lb, h->d_levels, level_launch(h, l)));
+      YGG_RETURN_IF_ERROR(accumulate_level(h, l, lb, h->d_levels, h->hist_plan[l]));
     }
     // after the collective this rank's statistics of the level sit in `level_stats`
     const unsigned long long* level_stats = lb.stats;
@@ -2659,17 +2622,17 @@ int ygg_tree_train_on_gradients(ygg_gbt* h, const float* gradients, const float*
 int ygg_debug_hist_plan(const ygg_gbt* h, int32_t level, ygg_hist_plan* out) {
   if (!h || !out) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (level < 0 || level >= h->num_levels) return set_error(YGG_ERR_INVALID_ARGUMENT, "level %d outside [0, %d)", level, h->num_levels);
+  const HistLaunch& pl = h->hist_plan[level];
   ygg_hist_plan p{};
-  if (h->hist2_FL[level] > 0) {
-    p.mode = YGG_HIST_HIST2; p.group = h->hist2_FL[level]; p.hist2_tiles = h->hist2_T[level];
+  if (pl.FL > 0) {
+    p.mode = YGG_HIST_HIST2; p.group = pl.FL; p.hist2_tiles = pl.T;
   } else {
-    const int m = h->hist_mode[level];
-    p.mode = m == kHistRootSum ? YGG_HIST_ROOT_SUM : m == kHistPacked ? YGG_HIST_PACKED : YGG_HIST_SHARED;
-    p.group = h->hist_G[level];
+    p.mode = pl.mode == kHistRootSum ? YGG_HIST_ROOT_SUM : pl.mode == kHistPacked ? YGG_HIST_PACKED : YGG_HIST_SHARED;
+    p.group = pl.G;
   }
-  p.chunk_blocks = h->hist_chunk[level];
-  p.slot_window = h->hist_passes[level] > 1 ? h->hist_S[level] - 1 : 0;
-  p.grid = h->hist_grid[level];
+  p.chunk_blocks = pl.chunk;
+  p.slot_window = pl.window;
+  p.grid = pl.grid;
   *out = p;
   return YGG_OK;
 }
@@ -2699,7 +2662,7 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
   // the launch, validated on the host: a plan the kernels cannot run exactly is refused, never launched
   HistLaunch pl{};
   if (plan == nullptr) {
-    pl = level_launch(h, level);
+    pl = h->hist_plan[level];
     if (n_slots > level_slot_bound(h, level))
       return set_error(YGG_ERR_INVALID_ARGUMENT, "the plan of level %d holds %d slots, %d requested", level, level_slot_bound(h, level), n_slots);
   } else {
@@ -2715,7 +2678,7 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
       if (p.hist2_tiles != 1 && p.hist2_tiles != 2) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2: %d sub-tiles (1 or 2)", p.hist2_tiles);
       if (p.slot_window != 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2 has no multi-pass form");
       if (n_slots > 2) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2 with %d slots (at most 2)", n_slots);
-      if (hist2_smem_bytes(p.group, n_slots, p.hist2_tiles, level == 0) > 216 * 1024)
+      if (hist2_smem_bytes(p.group, n_slots, p.hist2_tiles, level == 0) > kHist2SmemBudget)
         return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2 needs %zu bytes of shared memory (budget 216 KB)", hist2_smem_bytes(p.group, n_slots, p.hist2_tiles, level == 0));
       pl.FL = p.group; pl.T = p.hist2_tiles; pl.S = n_slots; pl.G = 1; pl.passes = 1;
       pl.mode = level == 0 ? kHistRootSum : kHistPacked;
@@ -2755,15 +2718,7 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
       return set_error(YGG_ERR_INVALID_ARGUMENT, "packed layout: a bin receives %u rows in one chunk of %d blocks (at most %u)", m, pl.chunk, kPackedMaxUpdates);
   }
   if (pl.mode == kHistRootSum) YGG_RETURN_IF_ERROR(ensure_root_counts(h));
-  if (pl.FL == 0) {   // the per-kernel shared-memory cap (configure_launches raises it only for the layouts the handle runs)
-    size_t budget = 0;
-    YGG_RETURN_IF_ERROR(hist_smem_budget(h->ds->device, &budget));
-    const int st = for_hist_kernel(hh, pl.mode, [&](auto kern) -> int {
-      YGG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(budget)));
-      return YGG_OK;
-    }, pl.window > 0);
-    if (st != YGG_OK) return st;
-  }
+  YGG_RETURN_IF_ERROR(raise_hist_smem_caps_once(h->ds->device));
 
   // Inputs in the training format.  Temporaries for everything the boosting state keeps (gradients, node ids, device
   // scalars, level descriptors, level buffer); the active lists, q24 / hq24 and act_sub are scratch every iteration rewrites.
