@@ -185,6 +185,18 @@ int ygg_dataset_set_feature_types(ygg_dataset* ds, const int32_t* feature_types,
  * `na_replacement` = the column mean the exact splitter imputes missing values with: na_value = na_replacement >= threshold
  * (splitter_accumulator.h:218). */
 int ygg_dataset_set_bucket_values(ygg_dataset* ds, int32_t feature, const float* values, int32_t n, float na_replacement);
+/* Wide numerical column (DESIGN.md §20): a numerical feature with num_bins = 257..65535 buckets, one per distinct value
+ * (the column mean is one more when it has missing values), that the byte columns cannot hold.  codes[r] < num_bins is the
+ * bucket of row r (missing values already folded into na_bin); values[b] = the value of bucket b (finite, strictly
+ * ascending); na_replacement = the column mean.  Such a feature is always split with the exact threshold rule of
+ * ygg_dataset_set_bucket_values: ygg_node.threshold_bin is a bucket index (compare it with the code), threshold_value the
+ * float threshold.  The feature's byte column becomes a one-bucket filler that the byte kernels never split on.  Call
+ * before ygg_gbt_create; single GPU only (the shard setters return YGG_ERR_UNIMPLEMENTED on such a dataset).  Training
+ * and validation / prediction datasets must have the same wide features and buckets. */
+int ygg_dataset_set_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
+                                const float* values, float na_replacement);
+/* Read-back of a wide column: codes[n_rows], and (may be NULL) its num_bins / na_bin. */
+int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t* codes, int32_t* num_bins, int32_t* na_bin);
 int ygg_dataset_destroy(ygg_dataset* ds);
 int64_t ygg_dataset_num_rows(const ygg_dataset* ds);
 int32_t ygg_dataset_num_features(const ygg_dataset* ds);
@@ -383,6 +395,12 @@ int ygg_debug_hist_plan(const ygg_gbt* h, int32_t level, ygg_hist_plan* out);
 int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* plan, const float* gradients,
                               const float* second, const int32_t* slot_of_row, int32_t n_slots, uint64_t* out_sum,
                               uint32_t* out_cnt, uint64_t* out_second, float* out_scales);
+
+/* The wide columns' histograms of the last histogram phase run on the handle (a training level, or
+ * ygg_debug_level_histogram, which accumulates them too): [n_slots][sum over the wide features of num_bins] raw sums of q,
+ * row counts and (exactly when the handle keeps one, else NULL) second-plane sums; the buckets of the wide features
+ * follow each other in the order they were set. */
+int ygg_debug_wide_histogram(ygg_gbt* h, int32_t n_slots, uint64_t* out_sum, uint32_t* out_cnt, uint64_t* out_second);
 
 /* SplitExamplesInPlace seam (learner/decision_tree/training.cc:5243-5305 ->
  * model/decision_tree/decision_tree.cc:957-1012): stable two-way partition of a row-id list by

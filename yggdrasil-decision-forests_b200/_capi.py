@@ -77,6 +77,7 @@ EXPORTS = [
     "ygg_dataset_get_bins", "ygg_dataset_set_bucket_values", "ygg_gbt_tie_stats", "ygg_gbt_set_tie_rng_position",
     "ygg_gbt_best_split_window_bytes", "ygg_gbt_set_best_split_window", "ygg_comm_window_create",
     "ygg_comm_unique_id", "ygg_comm_create", "ygg_comm_destroy", "ygg_comm_allreduce", "ygg_comm_allgather", "ygg_comm_reducescatter",
+    "ygg_dataset_set_wide_column", "ygg_dataset_get_wide_column", "ygg_debug_wide_histogram",
 ]
 
 
@@ -147,6 +148,29 @@ class Dataset:
         check(lib().ygg_dataset_set_bucket_values(self.handle, C.c_int32(int(feature)), ptr(v, C.c_float), C.c_int32(len(v)),
                                                   C.c_float(float(np.float32(na_replacement)))))
 
+    def set_wide_column(self, feature, codes, num_bins, na_bin, values, na_replacement):
+        """Wide numerical column (257..65535 buckets, one per distinct value): codes[r] = the uint16 bucket of row r,
+        values[b] = the value of bucket b, na_replacement = the column mean.  Always split with the exact threshold rule."""
+        c = np.ascontiguousarray(codes, dtype=np.uint16)
+        v = np.ascontiguousarray(values, dtype=np.float32)
+        if len(v) != int(num_bins):
+            raise ValueError(f"{len(v)} bucket values for {num_bins} buckets")
+        check(lib().ygg_dataset_set_wide_column(self.handle, C.c_int32(int(feature)), ptr(c, C.c_uint16), C.c_int64(len(c)),
+                                                C.c_int32(int(num_bins)), C.c_int32(int(na_bin)), ptr(v, C.c_float),
+                                                C.c_float(float(np.float32(na_replacement)))))
+        self.num_bins = self.num_bins.copy()
+        self.na_bin = self.na_bin.copy()
+        self.num_bins[feature], self.na_bin[feature] = 1, 0   # the byte column is a one-bucket filler
+        self.wide = dict(getattr(self, "wide", {}))
+        self.wide[int(feature)] = (int(num_bins), int(na_bin))
+
+    def get_wide_column(self, feature):
+        """-> (uint16 codes, num_bins, na_bin) of a wide column."""
+        out = np.empty(self.n_rows, np.uint16)
+        nb, na = C.c_int32(), C.c_int32()
+        check(lib().ygg_dataset_get_wide_column(self.handle, C.c_int32(int(feature)), ptr(out, C.c_uint16), C.byref(nb), C.byref(na)))
+        return out, nb.value, na.value
+
     def set_feature_types(self, feature_types):
         """feature_types[f]: FEATURE_DISCRETIZED_NUMERICAL or FEATURE_CATEGORICAL."""
         ft = np.ascontiguousarray(feature_types, dtype=np.int32)
@@ -169,6 +193,7 @@ class Dataset:
             d = Dataset.__new__(Dataset)
             d.handle, d.n_features, d.n_rows = hnd, self.n_features, n
             d.num_bins, d.na_bin, d.feature_types, d.h2d_bytes = self.num_bins, self.na_bin, self.feature_types, 0
+            d.wide = dict(getattr(self, "wide", {}))
             out.append(d)
         return out[0], out[1]
 
@@ -593,6 +618,17 @@ class Gbt:
                                               C.c_int32(n_slots), ptr(s, C.c_uint64), ptr(c, C.c_uint32),
                                               ptr(s2, C.c_uint64), ptr(scales, C.c_float)))
         return s, c, s2, (float(scales[0]), float(scales[1]))
+
+    def wide_histogram(self, n_slots):
+        """Raw wide-column histograms of the last histogram phase (a training level or level_histogram):
+        (sum u64, count u32, second-plane sum u64 or None), each [n_slots, sum of the wide features' buckets]."""
+        total = sum(nb for nb, _ in getattr(self.dataset, "wide", {}).values())
+        s = np.zeros((int(n_slots), total), np.uint64)
+        c = np.zeros((int(n_slots), total), np.uint32)
+        s2 = np.zeros((int(n_slots), total), np.uint64) if self.has_second_plane() else None
+        check(lib().ygg_debug_wide_histogram(self.handle, C.c_int32(int(n_slots)), ptr(s, C.c_uint64), ptr(c, C.c_uint32),
+                                             ptr(s2, C.c_uint64)))
+        return s, c, s2
 
     def has_second_plane(self):
         """True when the handle accumulates a second histogram plane: hessians (hessian gain with a logit loss) or

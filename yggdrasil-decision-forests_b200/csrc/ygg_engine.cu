@@ -28,6 +28,7 @@
 #include "ygg_internal.h"
 #include "../../include/ygg_b200_model.h"
 #include "ygg_kernels.cuh"
+#include "ygg_wide.cuh"
 
 using namespace ygg;
 
@@ -163,6 +164,20 @@ struct ygg_gbt {
   unsigned long long* d_hist_hsum[2] = {nullptr, nullptr};
   Candidate* d_cand = nullptr;
   uint32_t* d_cand_mask = nullptr;  // [split-level nodes][f_scan][8]
+  // wide columns (DESIGN.md §20): the level's slot planes [wide slots][wide_total], the per-node parent planes
+  // [split-level nodes][wide_total] (ping-pong like d_hist_*), the float thresholds of the wide candidates
+  int64_t wide_total = 0;
+  int wide_slots = 0;
+  bool counted = false;              // counted in ds->handles (a handle that failed to initialise is not)
+  unsigned long long* d_wsum = nullptr;
+  uint32_t* d_wcnt = nullptr;
+  unsigned long long* d_whsum = nullptr;
+  unsigned long long* d_wnode_sum[2] = {nullptr, nullptr};
+  uint32_t* d_wnode_cnt[2] = {nullptr, nullptr};
+  unsigned long long* d_wnode_hsum[2] = {nullptr, nullptr};
+  float* d_wide_thr = nullptr;       // [split-level nodes][f_scan]
+  int32_t* d_wide_feature = nullptr; // [wide features]
+  int32_t* d_wide_bins = nullptr;
   ShardBest* d_shard_best = nullptr;
   TieRec* d_ties = nullptr;        // [max level nodes] ties of the level being selected (single GPU)
   // stochastic gradient boosting (cfg.subsample < 1): this iteration's sample, drawn on the host from the learner's engine
@@ -598,6 +613,72 @@ int configure_launches(ygg_gbt* h) {
   return YGG_OK;
 }
 
+// Wide columns (DESIGN.md §20): (slots of the deepest split level + 2 x its nodes) x wide_total buckets x 12 B (20 B with
+// a second plane), once per handle.  A failed allocation is reported with the size it asked for.
+int allocate_wide_buffers(ygg_gbt* h) {
+  const ygg_dataset* ds = h->ds;
+  // (re)allocation, like allocate_level_buffers: ygg_gbt_set_weights runs it again when the handle gains a second plane
+  dev_free(h->d_wsum); dev_free(h->d_wcnt); dev_free(h->d_whsum);
+  h->d_wsum = nullptr; h->d_wcnt = nullptr; h->d_whsum = nullptr;
+  for (int i = 0; i < 2; i++) {
+    dev_free(h->d_wnode_sum[i]); dev_free(h->d_wnode_cnt[i]); dev_free(h->d_wnode_hsum[i]);
+    h->d_wnode_sum[i] = nullptr; h->d_wnode_cnt[i] = nullptr; h->d_wnode_hsum[i] = nullptr;
+  }
+  dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins);
+  h->d_wide_thr = nullptr; h->d_wide_feature = nullptr; h->d_wide_bins = nullptr;
+  h->wide_total = 0;
+  h->wide_slots = 0;
+  if (ds->n_wide() == 0 || h->num_levels == 0) return YGG_OK;
+  YGG_CUDA(cudaDeviceSynchronize());   // the freed planes go back to the pool before the new ones are taken
+  const int f_scan = h->f_end - h->f_begin;
+  h->wide_total = ds->wide_off.back();
+  h->wide_slots = level_slot_bound(h, h->num_levels - 1);
+  const size_t nodes = static_cast<size_t>(1) << std::max(0, h->num_levels - 1);
+  const bool hh = hist_hess(h);
+  const size_t per_bucket = sizeof(unsigned long long) + sizeof(uint32_t) + (hh ? sizeof(unsigned long long) : 0);
+  const size_t slot_elems = static_cast<size_t>(h->wide_slots) * h->wide_total, node_elems = nodes * h->wide_total;
+  auto fail = [&]() {
+    (void)cudaGetLastError();
+    return set_error(YGG_ERR_CUDA, "wide columns: %.2f GB of histogram planes ((%d slots + 2 x %zu nodes) x %lld buckets x %zu B) "
+                     "could not be allocated; lower max_depth or the buckets of the wide columns",
+                     static_cast<double>(slot_elems + 2 * node_elems) * per_bucket / 1e9, h->wide_slots, nodes,
+                     static_cast<long long>(h->wide_total), per_bucket);
+  };
+  if (dev_alloc(&h->d_wsum, slot_elems) != YGG_OK || dev_alloc(&h->d_wcnt, slot_elems) != YGG_OK ||
+      (hh && dev_alloc(&h->d_whsum, slot_elems) != YGG_OK))
+    return fail();
+  for (int i = 0; i < 2; i++)
+    if (dev_alloc(&h->d_wnode_sum[i], node_elems) != YGG_OK || dev_alloc(&h->d_wnode_cnt[i], node_elems) != YGG_OK ||
+        (hh && dev_alloc(&h->d_wnode_hsum[i], node_elems) != YGG_OK))
+      return fail();
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_thr, nodes * f_scan));
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_feature, ds->n_wide()));
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_bins, ds->n_wide()));
+  YGG_CUDA(cudaMemcpy(h->d_wide_feature, ds->wide_feature.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+  YGG_CUDA(cudaMemcpy(h->d_wide_bins, ds->wide_bins.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+  return YGG_OK;
+}
+
+// The wide columns' histogram phase of a level: zeroes the planes of `slots` slots and accumulates the level's active
+// lists into them (k_hist_wide).  grow_tree and ygg_debug_level_histogram both run it.
+int accumulate_wide(ygg_gbt* h, int slots) {
+  if (h->wide_total == 0) return YGG_OK;
+  const ygg_dataset* ds = h->ds;
+  const size_t elems = static_cast<size_t>(slots) * h->wide_total;
+  YGG_CUDA(cudaMemsetAsync(h->d_wsum, 0, elems * sizeof(unsigned long long), h->stream));
+  YGG_CUDA(cudaMemsetAsync(h->d_wcnt, 0, elems * sizeof(uint32_t), h->stream));
+  if (hist_hess(h)) YGG_CUDA(cudaMemsetAsync(h->d_whsum, 0, elems * sizeof(unsigned long long), h->stream));
+  WideHistParams wp{};
+  wp.wide = ds->d_wide; wp.n_pad = ds->n_pad; wp.off = ds->d_wide_off;
+  wp.act = h->d_act; wp.act_h = hist_hess(h) ? h->d_act_h : nullptr; wp.act_count = h->d_act_count; wp.n_blocks = h->n_blocks;
+  wp.total = h->wide_total; wp.sum = h->d_wsum; wp.cnt = h->d_wcnt; wp.hsum = hist_hess(h) ? h->d_whsum : nullptr;
+  // 8 CTAs of 256 threads per SM in all, spread over the wide features
+  const dim3 grid(static_cast<unsigned>(std::max(1, std::min(h->n_blocks, ds->num_sms * 8 / ds->n_wide()))), static_cast<unsigned>(ds->n_wide()));
+  k_hist_wide<<<grid, 256, 0, h->stream>>>(wp);
+  h->launches_total++;
+  return check_launch("k_hist_wide");
+}
+
 // (Re)allocates everything whose size depends on the feature shard.
 int allocate_level_buffers(ygg_gbt* h) {
   const int f_scan = h->f_end - h->f_begin;
@@ -629,7 +710,7 @@ int allocate_level_buffers(ygg_gbt* h) {
   (void)f_hist;
   h->level_buf_bytes = max_u64 * sizeof(unsigned long long);
   YGG_RETURN_IF_ERROR(dev_alloc_plain(&h->d_level_buf, max_u64));
-  return YGG_OK;
+  return allocate_wide_buffers(h);
 }
 
 int launch_hist(ygg_gbt* h, const HistParams& hp, int mode, int grid, size_t smem, bool multi = false) {
@@ -835,6 +916,10 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       ProfScope ps_level(h, kHistLevelNames[l & 15]);
       YGG_RETURN_IF_ERROR(accumulate_level(h, l, lb, h->d_levels, h->hist_plan[l]));
     }
+    if (h->wide_total > 0) {
+      ProfScope ps(h, "hist_wide");
+      YGG_RETURN_IF_ERROR(accumulate_wide(h, slots_of(l)));
+    }
     // after the collective this rank's statistics of the level sit in `level_stats`
     const unsigned long long* level_stats = lb.stats;
     if (rows_sharded && h->scatter) {
@@ -872,6 +957,22 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       else k_scan<false><<<grid, 256, 0, h->stream>>>(sc);
       h->launches_total++;
       YGG_RETURN_IF_ERROR(check_launch("k_scan"));
+      if (h->wide_total > 0) {   // after k_scan: overwrites its (never found) candidates of the wide features
+        ProfScope psw(h, "scan_wide");
+        WideScanParams wp{};
+        wp.s = sc;
+        wp.wide_feature = h->d_wide_feature; wp.wide_bins = h->d_wide_bins; wp.off = ds->d_wide_off; wp.values = ds->d_wide_values;
+        wp.total = h->wide_total;
+        wp.slot_sum = h->d_wsum; wp.slot_cnt = h->d_wcnt; wp.slot_hsum = h->d_whsum;
+        wp.node_sum = h->d_wnode_sum[par]; wp.node_cnt = h->d_wnode_cnt[par]; wp.node_hsum = h->d_wnode_hsum[par];
+        wp.pnode_sum = h->d_wnode_sum[par ^ 1]; wp.pnode_cnt = h->d_wnode_cnt[par ^ 1]; wp.pnode_hsum = h->d_wnode_hsum[par ^ 1];
+        wp.thr_value = h->d_wide_thr;
+        const dim3 wgrid(level_slot_bound(h, l), ds->n_wide());
+        if (hist_hess(h) || use_hess(h)) k_scan_wide<true><<<wgrid, 256, 0, h->stream>>>(wp);
+        else k_scan_wide<false><<<wgrid, 256, 0, h->stream>>>(wp);
+        h->launches_total++;
+        YGG_RETURN_IF_ERROR(check_launch("k_scan_wide"));
+      }
     }
     {
       ProfScope ps(h, "select");
@@ -889,6 +990,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       sel.max_depth = h->cfg.max_depth; sel.sibling_subtraction = h->cfg.sibling_subtraction;
       sel.max_slots = (l + 1 < h->num_levels) ? level_slot_bound(h, l + 1) : 0x7fffffff;
       sel.st = h->d_st; sel.max_nodes = h->max_nodes;
+      sel.wide_of = h->wide_total > 0 ? ds->d_wide_of : nullptr; sel.wide_thr_value = h->wide_total > 0 ? h->d_wide_thr : nullptr;
       const int threads = 256, blocks = (level_nodes_bound + (threads / 32) - 1) / (threads / 32);
       k_select_local<<<blocks, threads, 0, h->stream>>>(sel);
       h->launches_total++;
@@ -937,8 +1039,16 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       const int per_cta = (h->n_blocks + h->ds->num_sms * 2 - 1) / (h->ds->num_sms * 2);
       const bool any_cat = std::any_of(ds->feature_type.begin(), ds->feature_type.end(),
                                        [](int32_t t) { return t == YGG_FEATURE_CATEGORICAL; });
-      if (any_cat) k_partition<true><<<(h->n_blocks + per_cta - 1) / per_cta, kPartThreads, smem, h->stream>>>(pp);
-      else k_partition<false><<<(h->n_blocks + per_cta - 1) / per_cta, kPartThreads, smem, h->stream>>>(pp);
+      const int pgrid = (h->n_blocks + per_cta - 1) / per_cta;
+      if (ds->n_wide() > 0) {   // the byte-only instantiations stay as they are for datasets without wide columns
+        pp.wide = ds->d_wide; pp.wide_of = ds->d_wide_of;
+        if (any_cat) k_partition_wide<true><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
+        else k_partition_wide<false><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
+      } else if (any_cat) {
+        k_partition<true><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
+      } else {
+        k_partition<false><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
+      }
       h->launches_total++;
       YGG_RETURN_IF_ERROR(check_launch("k_partition"));
       if (l + 1 < h->num_levels) YGG_RETURN_IF_ERROR(replicate_stats(h, lbn, children_bound));
@@ -956,7 +1066,8 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
   if (h->cfg.candidate_shuffle != 0 && h->world == 1) {
     // which of the tied candidates recorded by k_select_local cut their node's rows exactly like the chosen split
     ProfScope ps(h, "select");
-    k_verify_ties<<<elementwise_grid(h), 256, 0, h->stream>>>(nodes, h->d_node_of_row, ds->d_bins, ds->n, ds->n_pad);
+    k_verify_ties<<<elementwise_grid(h), 256, 0, h->stream>>>(nodes, h->d_node_of_row, ds->d_bins, ds->n, ds->n_pad, ds->d_wide,
+                                                              ds->n_wide() > 0 ? ds->d_wide_of : nullptr);
     h->launches_total++;
     YGG_RETURN_IF_ERROR(check_launch("k_verify_ties"));
   }
@@ -1086,8 +1197,16 @@ __global__ void __launch_bounds__(256) k_apply_leaves(float* __restrict__ pred, 
 // Validation rows: UpdatePredictions on the held-out rows by tree traversal (loss_utils.cc:214-229,
 // gradient_boosted_trees.cc:1556-1566) fused with the validation loss of the iteration
 // (:1610-1626; loss_imp_binomial.cc:204-234, metric/metric.cc:2173-2199).
+// The bucket of row r of feature f: its uint16 code for a wide column (`wide_of` null: the dataset has none), else its byte.
+__device__ __forceinline__ uint32_t row_bin(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
+                                            const int32_t* __restrict__ wide_of, int64_t n_pad, int f, int64_t r) {
+  const int wi = wide_of != nullptr ? wide_of[f] : -1;
+  return wi >= 0 ? wide[static_cast<int64_t>(wi) * n_pad + r] : bins[static_cast<int64_t>(f) * n_pad + r];
+}
+
 template <int LOSS>
-__global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict__ bins, int64_t n, int64_t n_pad,
+__global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
+                                                      const int32_t* __restrict__ wide_of, int64_t n, int64_t n_pad,
                                                       const NodeRec* __restrict__ tree, float* __restrict__ pred,
                                                       const uint8_t* __restrict__ label_u8,
                                                       const float* __restrict__ label_f32, LossRec* out, LossPartials* partials,
@@ -1100,7 +1219,7 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
     while (true) {
       const int f = tree[node].feature;
       if (f < 0) break;
-      const uint32_t b = bins[static_cast<int64_t>(f) * n_pad + r];
+      const uint32_t b = row_bin(bins, wide, wide_of, n_pad, f, r);
       const bool pos = tree[node].cond_type == 1 ? ((tree[node].mask[b >> 5] >> (b & 31)) & 1u) != 0
                                                  : static_cast<int>(b) >= tree[node].thr;
       node = pos ? tree[node].pos_child : tree[node].neg_child;
@@ -1141,7 +1260,8 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
 // Raw scores of the model's first `n_trees` trees on any dataset with the training dataset's features (ComputePredictions,
 // gradient_boosted_trees.cc:2872-2930: the predictions a resumed training starts from): initial prediction + the leaves
 // reached in every tree of the row's class plane.  One thread per row, trees in order (float sums in the reference's order).
-__global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bins, int64_t n, int64_t n_pad, const NodeRec* __restrict__ trees,
+__global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
+                                                const int32_t* __restrict__ wide_of, int64_t n, int64_t n_pad, const NodeRec* __restrict__ trees,
                                                 int max_nodes, int n_trees, int K, float initial, float* __restrict__ out /*[K][n]*/) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n; r += stride) {
@@ -1153,7 +1273,7 @@ __global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bin
         while (true) {
           const int f = tree[node].feature;
           if (f < 0) break;
-          const uint32_t b = bins[static_cast<int64_t>(f) * n_pad + r];
+          const uint32_t b = row_bin(bins, wide, wide_of, n_pad, f, r);
           const bool pos = tree[node].cond_type == 1 ? ((tree[node].mask[b >> 5] >> (b & 31)) & 1u) != 0
                                                      : static_cast<int>(b) >= tree[node].thr;
           node = pos ? tree[node].pos_child : tree[node].neg_child;
@@ -1173,7 +1293,7 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
   const int64_t nv = h->vds->n;
   const int grid = static_cast<int>(std::min<int64_t>((nv + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 8));
   if (is_multinomial(h)) {
-    k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, nv, h->vds->n_pad, tree, h->d_vpred + static_cast<int64_t>(plane) * nv,
+    k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, h->d_vpred + static_cast<int64_t>(plane) * nv,
                                                    nullptr, nullptr, nullptr, nullptr, nullptr, 0.f);
     h->launches_total++;
     YGG_RETURN_IF_ERROR(check_launch("k_valid_update"));
@@ -1190,11 +1310,11 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
     return YGG_OK;
   }
   if (h->cfg.loss == YGG_LOSS_BINOMIAL_LOG_LIKELIHOOD)
-    k_valid_update<0><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, nv, h->vds->n_pad, tree, h->d_vpred, h->d_vlabel_u8,
+    k_valid_update<0><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, h->d_vpred, h->d_vlabel_u8,
                                                    h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
                                                    h->d_vweight, h->v_correct_scale);
   else
-    k_valid_update<1><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, nv, h->vds->n_pad, tree, h->d_vpred, h->d_vlabel_u8,
+    k_valid_update<1><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, h->d_vpred, h->d_vlabel_u8,
                                                    h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
                                                    h->d_vweight, h->v_correct_scale);
   h->launches_total++;
@@ -1720,9 +1840,104 @@ int ygg_dataset_set_bucket_values(ygg_dataset* ds, int32_t feature, const float*
   return YGG_OK;
 }
 
+namespace {
+// (Re)uploads the wide columns' tables from their host copies.
+int upload_wide_meta(ygg_dataset* ds) {
+  dev_free(ds->d_wide_of); dev_free(ds->d_wide_off); dev_free(ds->d_wide_values);
+  ds->d_wide_of = nullptr; ds->d_wide_off = nullptr; ds->d_wide_values = nullptr;
+  YGG_RETURN_IF_ERROR(dev_alloc(&ds->d_wide_of, ds->F));
+  YGG_RETURN_IF_ERROR(dev_alloc(&ds->d_wide_off, ds->wide_off.size()));
+  YGG_RETURN_IF_ERROR(dev_alloc(&ds->d_wide_values, ds->wide_values.size()));
+  YGG_CUDA(cudaMemcpy(ds->d_wide_of, ds->wide_of.data(), sizeof(int32_t) * ds->F, cudaMemcpyHostToDevice));
+  YGG_CUDA(cudaMemcpy(ds->d_wide_off, ds->wide_off.data(), sizeof(int64_t) * ds->wide_off.size(), cudaMemcpyHostToDevice));
+  YGG_CUDA(cudaMemcpy(ds->d_wide_values, ds->wide_values.data(), sizeof(float) * ds->wide_values.size(), cudaMemcpyHostToDevice));
+  return YGG_OK;
+}
+// The NA replacement of the features under an exact threshold rule lives in d_na_replacement [F] (with d_bucket_values /
+// d_exact_rule, allocated on first use), wide columns included: k_select_* read it for both.
+int ensure_exact_arrays(ygg_dataset* ds) {
+  if (ds->d_bucket_values != nullptr) return YGG_OK;
+  YGG_RETURN_IF_ERROR(dev_alloc(&ds->d_bucket_values, static_cast<size_t>(ds->F) * kMaxBins));
+  YGG_RETURN_IF_ERROR(dev_alloc(&ds->d_exact_rule, ds->F));
+  return dev_alloc(&ds->d_na_replacement, ds->F);
+}
+}  // namespace
+
+int ygg_dataset_set_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
+                                const float* values, float na_replacement) {
+  // the checks that need no dataset first (they hold without a device too), then those against the dataset
+  if (!codes || !values) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (num_bins < kMaxBins + 1 || num_bins > 65535)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: num_bins=%d outside [257, 65535] (fewer fit the byte columns)", feature, num_bins);
+  if (na_bin < 0 || na_bin >= num_bins) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: na_bin=%d outside [0, num_bins)", feature, na_bin);
+  if (n < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "negative row count %lld", static_cast<long long>(n));
+  for (int i = 0; i < num_bins; i++)
+    if (!std::isfinite(values[i]) || (i > 0 && !(values[i] > values[i - 1])))
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: bucket values must be finite and strictly ascending", feature);
+  for (int64_t r = 0; r < n; r++)
+    if (codes[r] >= num_bins)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: code %u of row %lld >= num_bins=%d", feature, codes[r], static_cast<long long>(r), num_bins);
+  if (!ds) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
+  if (ds->handles > 0)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "wide columns are set before ygg_gbt_create: %d handle(s) already use this dataset", ds->handles);
+  if (ds->feature_type[feature] != YGG_FEATURE_DISCRETIZED_NUMERICAL)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is categorical: wide columns are numerical", feature);
+  if (!ds->wide_of.empty() && ds->wide_of[feature] >= 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is already a wide column", feature);
+  if (n != ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "%lld codes for a dataset of %lld rows", static_cast<long long>(n), static_cast<long long>(ds->n));
+  YGG_RETURN_IF_ERROR(require_device());
+  YGG_CUDA(cudaSetDevice(ds->device));
+  const int W = ds->n_wide();
+  // the code matrix grows by one plane (the old planes are copied over)
+  uint16_t* grown = nullptr;
+  YGG_RETURN_IF_ERROR(dev_alloc(&grown, static_cast<size_t>(W + 1) * ds->n_pad));
+  if (W > 0) YGG_CUDA(cudaMemcpy(grown, ds->d_wide, sizeof(uint16_t) * W * ds->n_pad, cudaMemcpyDeviceToDevice));
+  YGG_CUDA(cudaMemcpy(grown + static_cast<size_t>(W) * ds->n_pad, codes, sizeof(uint16_t) * n, cudaMemcpyHostToDevice));
+  dev_free(ds->d_wide);
+  ds->d_wide = grown;
+  // the byte column: a filler over all 256 bins with one bucket, i.e. never a valid split for k_scan.  (All rows in one
+  // bin would be as good for the scan, but would push k_hist's packed layout, whose bins take at most 8191 rows per work
+  // item, to its slower carry layout.)
+  std::vector<uint8_t> filler(n);
+  for (int64_t r = 0; r < n; r++) filler[r] = static_cast<uint8_t>(r & 0xFF);
+  YGG_CUDA(cudaMemcpy(ds->d_bins + static_cast<int64_t>(feature) * ds->n_pad, filler.data(), n, cudaMemcpyHostToDevice));
+  dev_free(ds->d_bins4);   // k_hist2's interleaved copy is rebuilt on first use
+  ds->d_bins4 = nullptr;
+  ds->num_bins[feature] = 1;
+  ds->na_bin[feature] = 0;
+  YGG_RETURN_IF_ERROR(ygg_internal_dataset_finalize(ds));
+  if (ds->wide_of.empty()) { ds->wide_of.assign(ds->F, -1); ds->wide_off.assign(1, 0); }
+  ds->wide_of[feature] = W;
+  ds->wide_feature.push_back(feature);
+  ds->wide_bins.push_back(num_bins);
+  ds->wide_na_bin.push_back(na_bin);
+  ds->wide_na_replacement.push_back(na_replacement);
+  ds->wide_values.insert(ds->wide_values.end(), values, values + num_bins);
+  ds->wide_off.push_back(ds->wide_off.back() + num_bins);
+  YGG_RETURN_IF_ERROR(upload_wide_meta(ds));
+  YGG_RETURN_IF_ERROR(ensure_exact_arrays(ds));
+  const int32_t zero = 0;
+  YGG_CUDA(cudaMemcpy(ds->d_exact_rule + feature, &zero, sizeof(zero), cudaMemcpyHostToDevice));
+  YGG_CUDA(cudaMemcpy(ds->d_na_replacement + feature, &na_replacement, sizeof(float), cudaMemcpyHostToDevice));
+  return YGG_OK;
+}
+
+int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t* codes, int32_t* num_bins, int32_t* na_bin) {
+  if (!ds || !codes) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
+  if (ds->wide_of.empty() || ds->wide_of[feature] < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is not a wide column", feature);
+  const int w = ds->wide_of[feature];
+  YGG_CUDA(cudaSetDevice(ds->device));
+  YGG_CUDA(cudaMemcpy(codes, ds->d_wide + static_cast<size_t>(w) * ds->n_pad, sizeof(uint16_t) * ds->n, cudaMemcpyDeviceToHost));
+  if (num_bins) *num_bins = ds->wide_bins[w];
+  if (na_bin) *na_bin = ds->wide_na_bin[w];
+  return YGG_OK;
+}
+
 int ygg_dataset_destroy(ygg_dataset* ds) {
   if (!ds) return YGG_OK;
   cudaSetDevice(ds->device);
+  dev_free(ds->d_wide); dev_free(ds->d_wide_of); dev_free(ds->d_wide_off); dev_free(ds->d_wide_values);
   dev_free(ds->d_bins);
   dev_free(ds->d_bins4);
   dev_free(ds->d_num_bins);
@@ -1808,6 +2023,8 @@ int ygg_gbt_create(ygg_gbt** out, ygg_dataset* ds, const ygg_gbt_config* cfg) {
     g_last_error = msg;
     return status;
   }
+  ds->handles++;
+  h->counted = true;
   *out = h;
   return YGG_OK;
 }
@@ -1890,6 +2107,7 @@ static int init_handle(ygg_gbt* h) {
 int ygg_gbt_destroy(ygg_gbt* h) {
   if (!h) return YGG_OK;
   cudaSetDevice(h->ds->device);
+  if (h->counted) h->ds->handles--;
   if (h->stream) cudaStreamSynchronize(h->stream);
   collect_profile(h);
   dev_free(h->d_label_u8); dev_free(h->d_label_f32); dev_free(h->d_pred); dev_free(h->d_g); dev_free(h->d_h);
@@ -1904,6 +2122,9 @@ int ygg_gbt_destroy(ygg_gbt* h) {
   dev_free(h->d_weight); dev_free(h->d_g2w); dev_free(h->d_wsums); dev_free(h->d_vweight);
   for (int i = 0; i < 2; i++) { dev_free(h->d_goss_keys[i]); dev_free(h->d_goss_rows[i]); }
   dev_free(h->d_goss_u);
+  dev_free(h->d_wsum); dev_free(h->d_wcnt); dev_free(h->d_whsum);
+  for (int i = 0; i < 2; i++) { dev_free(h->d_wnode_sum[i]); dev_free(h->d_wnode_cnt[i]); dev_free(h->d_wnode_hsum[i]); }
+  dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins);
   cudaFree(h->d_goss_temp);
   cudaFree(h->d_level_buf);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -2099,6 +2320,7 @@ int ygg_gbt_set_validation_weights_f32(ygg_gbt* h, const float* weights, int64_t
 int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature_end, int32_t rank,
                               int32_t world, ygg_allgather_fn exchange, void* ctx) {
   if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
+  if (h->ds->n_wide() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "wide columns (ygg_dataset_set_wide_column) are single GPU: not combined with feature shards");
   if (feature_begin < 0 || feature_end > h->ds->F || feature_begin >= feature_end)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "bad feature shard [%d, %d) of %d", feature_begin, feature_end, h->ds->F);
   if (world < 1 || rank < 0 || rank >= world) return set_error(YGG_ERR_INVALID_ARGUMENT, "bad rank %d / world %d", rank, world);
@@ -2121,6 +2343,7 @@ int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature
 int ygg_gbt_set_row_shard(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_rows_global,
                           float initial_prediction, ygg_allreduce_fn allreduce, void* ctx) {
   if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
+  if (h->ds->n_wide() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "wide columns (ygg_dataset_set_wide_column) are single GPU: not combined with row shards");
   if (world < 1 || rank < 0 || rank >= world) return set_error(YGG_ERR_INVALID_ARGUMENT, "bad rank %d / world %d", rank, world);
   if (world > 1 && !allreduce) return set_error(YGG_ERR_INVALID_ARGUMENT, "world > 1 needs an all-reduce function");
   if (n_rows_global < h->ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "n_rows_global < local rows");
@@ -2159,6 +2382,7 @@ int ygg_gbt_set_row_shard_scatter(ygg_gbt* h, int32_t rank, int32_t world, int64
                                   float initial_prediction, ygg_allreduce_fn allreduce,
                                   ygg_reducescatter_fn reducescatter, ygg_allgather_fn allgather, void* ctx) {
   if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
+  if (h->ds->n_wide() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "wide columns (ygg_dataset_set_wide_column) are single GPU: not combined with row shards");
   if (world > 1 && (!reducescatter || !allgather)) return set_error(YGG_ERR_INVALID_ARGUMENT, "world > 1 needs reduce-scatter and all-gather functions");
   if (world > h->ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "more ranks (%d) than features (%d)", world, h->ds->F);
   YGG_RETURN_IF_ERROR(ygg_gbt_set_row_shard(h, rank, world, n_rows_global, initial_prediction, allreduce, ctx));
@@ -2189,6 +2413,14 @@ __global__ void k_gather_rows(const uint8_t* __restrict__ in, int64_t in_pad, co
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_out; i += stride)
     out[static_cast<int64_t>(f) * out_pad + i] = in[static_cast<int64_t>(f) * in_pad + rows[i]];
 }
+// the same for the wide columns' uint16 planes
+__global__ void k_gather_rows16(const uint16_t* __restrict__ in, int64_t in_pad, const uint32_t* __restrict__ rows, int64_t n_out,
+                                int64_t out_pad, uint16_t* __restrict__ out) {
+  const int f = blockIdx.y;
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_out; i += stride)
+    out[static_cast<int64_t>(f) * out_pad + i] = in[static_cast<int64_t>(f) * in_pad + rows[i]];
+}
 
 int attach_validation(ygg_gbt* h, const ygg_dataset* valid, int64_t n) {
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
@@ -2196,7 +2428,8 @@ int attach_validation(ygg_gbt* h, const ygg_dataset* valid, int64_t n) {
   if (h->shard_mode != kShardNone) return set_error(YGG_ERR_UNIMPLEMENTED, "validation rows are not combined with sharding");
   if (!h->has_labels) return set_error(YGG_ERR_INVALID_ARGUMENT, "set the training labels first (the initial prediction comes from them)");
   if (valid->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset lives on another device");
-  if (valid->F != h->ds->F || valid->num_bins != h->ds->num_bins || valid->feature_type != h->ds->feature_type)
+  if (valid->F != h->ds->F || valid->num_bins != h->ds->num_bins || valid->feature_type != h->ds->feature_type ||
+      valid->wide_feature != h->ds->wide_feature || valid->wide_bins != h->ds->wide_bins)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset does not have the features / binning of the training dataset");
   if (n != valid->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "label count %lld != validation rows %lld", static_cast<long long>(n), static_cast<long long>(valid->n));
   YGG_CUDA(cudaSetDevice(h->ds->device));
@@ -2247,7 +2480,18 @@ int ygg_dataset_split_rows(const ygg_dataset* ds, const uint8_t* select, ygg_dat
     }
     dim3 grid(static_cast<unsigned>(std::min<int64_t>((n + 255) / 256, 2048)), static_cast<unsigned>(ds->F));
     k_gather_rows<<<grid, 256>>>(ds->d_bins, ds->n_pad, d_rows, n, out[k]->n_pad, out[k]->d_bins);
-    if (cudaDeviceSynchronize() != cudaSuccess) st = set_error(YGG_ERR_CUDA, "row gather failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (ds->n_wide() > 0) {   // the wide columns travel with the rows: codes, bucket values and NA replacements
+      ygg_dataset* o = out[k];
+      o->wide_of = ds->wide_of; o->wide_feature = ds->wide_feature; o->wide_bins = ds->wide_bins; o->wide_na_bin = ds->wide_na_bin;
+      o->wide_off = ds->wide_off; o->wide_values = ds->wide_values; o->wide_na_replacement = ds->wide_na_replacement;
+      st = dev_alloc(&o->d_wide, static_cast<size_t>(ds->n_wide()) * o->n_pad);
+      if (st == YGG_OK) st = upload_wide_meta(o);
+      if (st == YGG_OK) {
+        dim3 wgrid(grid.x, static_cast<unsigned>(ds->n_wide()));
+        k_gather_rows16<<<wgrid, 256>>>(ds->d_wide, ds->n_pad, d_rows, n, o->n_pad, o->d_wide);
+      }
+    }
+    if (st == YGG_OK && cudaDeviceSynchronize() != cudaSuccess) st = set_error(YGG_ERR_CUDA, "row gather failed: %s", cudaGetErrorString(cudaGetLastError()));
     cudaFree(d_rows);
     d_rows = nullptr;
     if (st == YGG_OK) st = ygg_internal_dataset_finalize(out[k]);
@@ -2561,7 +2805,8 @@ int ygg_gbt_get_predictions(ygg_gbt* h, float* out, int64_t n) {
 int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   if (!h || !ds || !out) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (ds->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset lives on another device");
-  if (ds->F != h->ds->F || ds->num_bins != h->ds->num_bins || ds->feature_type != h->ds->feature_type)
+  if (ds->F != h->ds->F || ds->num_bins != h->ds->num_bins || ds->feature_type != h->ds->feature_type ||
+      ds->wide_feature != h->ds->wide_feature || ds->wide_bins != h->ds->wide_bins)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset does not have the features / binning of the training dataset");
   if (n != ds->n * h->K) return set_error(YGG_ERR_INVALID_ARGUMENT, "n mismatch (rows x classes expected)");
   YGG_CUDA(cudaSetDevice(h->ds->device));
@@ -2571,7 +2816,7 @@ int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   YGG_RETURN_IF_ERROR(dev_alloc(&d_out, static_cast<size_t>(n)));
   const int n_trees = ygg_gbt_num_trees(h);
   k_predict<<<static_cast<int>(std::min<int64_t>((ds->n + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 16)), 256, 0, h->stream>>>(
-      ds->d_bins, ds->n, ds->n_pad, h->d_nodes_all, h->max_nodes, n_trees, h->K, h->initial_prediction, d_out);
+      ds->d_bins, ds->d_wide, ds->d_wide_of, ds->n, ds->n_pad, h->d_nodes_all, h->max_nodes, n_trees, h->K, h->initial_prediction, d_out);
   h->launches_total++;
   int st = check_launch("k_predict");
   if (st == YGG_OK && (cudaMemcpyAsync(out, d_out, sizeof(float) * n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
@@ -2703,6 +2948,8 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
     return set_error(YGG_ERR_INVALID_ARGUMENT, "a second histogram plane is accumulated by the shared layout only");
   if (pl.mode == kHistRootSum && (level != 0 || sampling(h) || !all_slot0 || n_slots != 1))
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the root layouts need level 0, no row sampling and every row in slot 0");
+  if (h->wide_total > 0 && n_slots > h->wide_slots)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "the wide-column planes of this handle hold %d slots, %d requested", h->wide_slots, n_slots);
   YGG_CUDA(cudaSetDevice(h->ds->device));
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
   if (pl.mode == kHistPacked) {   // k_hist packed words, or k_hist2 below the root
@@ -2772,6 +3019,7 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
     h->launches_total += 4;
     const LevelBuf lb = level_buf(h, n_slots, 1, d_buf);
     YGG_RETURN_IF_ERROR(accumulate_level(h, level, lb, d_lv, pl));
+    YGG_RETURN_IF_ERROR(accumulate_wide(h, n_slots));   // (read back with ygg_debug_wide_histogram)
     std::vector<unsigned long long> buf(lb.total_u64);
     DeviceState st;
     YGG_CUDA(cudaMemcpyAsync(buf.data(), d_buf, lb.total_u64 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
@@ -2800,6 +3048,23 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
   return status;
 }
 
+int ygg_debug_wide_histogram(ygg_gbt* h, int32_t n_slots, uint64_t* out_sum, uint32_t* out_cnt, uint64_t* out_second) {
+  if (!h || !out_sum || !out_cnt) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (h->wide_total == 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "the handle's dataset has no wide columns");
+  if (n_slots < 1 || n_slots > h->wide_slots) return set_error(YGG_ERR_INVALID_ARGUMENT, "n_slots=%d outside [1, %d]", n_slots, h->wide_slots);
+  const bool hh = hist_hess(h);
+  if (hh != (out_second != nullptr))
+    return set_error(YGG_ERR_INVALID_ARGUMENT, hh ? "this handle keeps a second histogram plane: `out_second` is required"
+                                                  : "this handle keeps no second histogram plane: `out_second` must be NULL");
+  YGG_CUDA(cudaSetDevice(h->ds->device));
+  const size_t elems = static_cast<size_t>(n_slots) * h->wide_total;
+  YGG_CUDA(cudaMemcpyAsync(out_sum, h->d_wsum, elems * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
+  YGG_CUDA(cudaMemcpyAsync(out_cnt, h->d_wcnt, elems * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  if (hh) YGG_CUDA(cudaMemcpyAsync(out_second, h->d_whsum, elems * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
+  YGG_CUDA(cudaStreamSynchronize(h->stream));
+  return YGG_OK;
+}
+
 int ygg_partition_rows(ygg_dataset* ds, const uint32_t* rows_in, int64_t n, int32_t feature,
                        int32_t threshold_bin, uint32_t* rows_out, int64_t* n_pos) {
   if (!ds || !rows_in || !rows_out || !n_pos) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
@@ -2817,15 +3082,19 @@ int ygg_partition_rows(ygg_dataset* ds, const uint32_t* rows_in, int64_t n, int3
   YGG_RETURN_IF_ERROR(dev_alloc(&d_out, n));
   YGG_RETURN_IF_ERROR(dev_alloc(&d_cnt, blocks));
   YGG_CUDA(cudaMemcpy(d_in, rows_in, n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  const int wi = ds->wide_of.empty() ? -1 : ds->wide_of[feature];
   const uint8_t* col = ds->d_bins + static_cast<int64_t>(feature) * ds->n_pad;
-  k_partition_count<<<blocks, 256>>>(col, d_in, n, threshold_bin, d_cnt);
+  const uint16_t* col16 = wi >= 0 ? ds->d_wide + static_cast<int64_t>(wi) * ds->n_pad : nullptr;   // a wide column's codes
+  if (col16 != nullptr) k_partition_count<<<blocks, 256>>>(col16, d_in, n, threshold_bin, d_cnt);
+  else k_partition_count<<<blocks, 256>>>(col, d_in, n, threshold_bin, d_cnt);
   YGG_RETURN_IF_ERROR(check_launch("k_partition_count"));
   std::vector<uint32_t> cnt(blocks);
   YGG_CUDA(cudaMemcpy(cnt.data(), d_cnt, blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   uint32_t total = 0;
   for (int i = 0; i < blocks; i++) { const uint32_t c = cnt[i]; cnt[i] = total; total += c; }
   YGG_CUDA(cudaMemcpy(d_cnt, cnt.data(), blocks * sizeof(uint32_t), cudaMemcpyHostToDevice));
-  k_partition_scatter<<<blocks, 256>>>(col, d_in, n, threshold_bin, d_cnt, total, d_out);
+  if (col16 != nullptr) k_partition_scatter<<<blocks, 256>>>(col16, d_in, n, threshold_bin, d_cnt, total, d_out);
+  else k_partition_scatter<<<blocks, 256>>>(col, d_in, n, threshold_bin, d_cnt, total, d_out);
   YGG_RETURN_IF_ERROR(check_launch("k_partition_scatter"));
   YGG_CUDA(cudaMemcpy(rows_out, d_out, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
   dev_free(d_in); dev_free(d_out); dev_free(d_cnt);

@@ -21,6 +21,17 @@ struct ygg_dataset {
   float* d_na_replacement = nullptr;  // [F] NumericalSpec.mean of the features under the exact rule
   std::vector<int32_t> num_bins, na_bin, feature_type;
   int num_sms = 0;
+  // Wide numerical columns (ygg_dataset_set_wide_column, DESIGN.md §20): 257..65535 buckets, uint16 codes.  The feature's
+  // byte column in d_bins holds a filler with num_bins[f] = 1, so the byte kernels never split on it.
+  uint16_t* d_wide = nullptr;          // [wide features][n_pad] codes, in wide-index order
+  int32_t* d_wide_of = nullptr;        // [F] wide index of a feature, -1 for a byte column
+  int64_t* d_wide_off = nullptr;       // [wide features] offset of the feature's buckets in d_wide_values / the wide planes
+  float* d_wide_values = nullptr;      // [sum of the wide features' buckets] bucket values (ascending per feature)
+  std::vector<int32_t> wide_of, wide_feature, wide_bins, wide_na_bin;
+  std::vector<int64_t> wide_off;       // host copy of d_wide_off, plus the total at the end
+  std::vector<float> wide_values, wide_na_replacement;
+  int n_wide() const { return static_cast<int>(wide_feature.size()); }
+  int handles = 0;                     // live ygg_gbt handles on this dataset (wide columns are set before the first)
 };
 
 __attribute__((visibility("hidden"))) int ygg_internal_dataset_alloc(ygg_dataset** out, int64_t n_rows,

@@ -402,21 +402,14 @@ __device__ __forceinline__ Scan3 block_inclusive_scan(Scan3 v, Scan3* s_warp /*[
   return v;
 }
 
-// Scans one node's 256-bin histogram held one bin per thread; thread 0 writes the Candidate.
-__device__ void scan_node(const ScanParams& p, const NodeRec& node, int f_global, long long cnt,
-                          long long sq /*unbiased quantised sum*/, long long hq, Candidate* out) {
-  __shared__ Scan3 s_warp[8];
-  __shared__ double s_best_score[8];
-  __shared__ int s_best_b[8];
-  __shared__ int s_interp[8];
-  const int b = threadIdx.x;
-  const int B = p.num_bins[f_global];
-  Scan3 tot;
-  const Scan3 inc = block_inclusive_scan(Scan3{cnt, sq, hq}, s_warp, &tot);
-  const double ginv = static_cast<double>(p.st->g_pow2) / static_cast<double>(1u << (kQBits - 1));
-  const double hinv = static_cast<double>(p.st->h_pow2) / static_cast<double>(1u << kQBits);
+// Score of the numerical boundary whose negative side holds the sums `inc` of a node with the sums `tot` (bucket
+// interpolation aside, ScanSplits' per-boundary step, splitter_scanner.h:931-1101) in *score_out; false when it is not a
+// valid split: `in_range` false (the last bucket), a side below min_num_obs rows (or without weight), or a score not above
+// the minimum.  Shared by the byte scan (scan_node) and the wide-column scan (k_scan_wide, ygg_wide.cuh).
+__device__ __forceinline__ bool boundary_score(const ScanParams& p, const Scan3& tot, const Scan3& inc, bool in_range,
+                                               double ginv, double hinv, double* score_out) {
   const long long n_neg = inc.c, n_pos = tot.c - inc.c;
-  bool valid = (b <= B - 2) && (n_pos >= p.min_num_obs) && (n_neg >= p.min_num_obs);
+  bool valid = in_range && (n_pos >= p.min_num_obs) && (n_neg >= p.min_num_obs);
   double score = 0.0;
   double min_score = 0.0;
   if (!p.use_hessian) {
@@ -467,6 +460,26 @@ __device__ void scan_node(const ScanParams& p, const NodeRec& node, int f_global
   }
   // best_score starts at max(condition.split_score (0), MinimumScore()) and needs strict '>'.
   valid = valid && (score > min_score) && (score > 0.0 || p.use_hessian);
+  *score_out = score;
+  return valid;
+}
+
+// Scans one node's 256-bin histogram held one bin per thread; thread 0 writes the Candidate.
+__device__ void scan_node(const ScanParams& p, const NodeRec& node, int f_global, long long cnt,
+                          long long sq /*unbiased quantised sum*/, long long hq, Candidate* out) {
+  __shared__ Scan3 s_warp[8];
+  __shared__ double s_best_score[8];
+  __shared__ int s_best_b[8];
+  __shared__ int s_interp[8];
+  const int b = threadIdx.x;
+  const int B = p.num_bins[f_global];
+  Scan3 tot;
+  const Scan3 inc = block_inclusive_scan(Scan3{cnt, sq, hq}, s_warp, &tot);
+  const double ginv = static_cast<double>(p.st->g_pow2) / static_cast<double>(1u << (kQBits - 1));
+  const double hinv = static_cast<double>(p.st->h_pow2) / static_cast<double>(1u << kQBits);
+  const long long n_pos = tot.c - inc.c;
+  double score;
+  const bool valid = boundary_score(p, tot, inc, b <= B - 2, ginv, hinv, &score);
   // arg-max with the lowest bin on ties (sequential strict '>' keeps the first maximum).
   double bs = valid ? score : -1.0;
   int bb = valid ? b : 0x7fffffff;
@@ -733,7 +746,18 @@ struct SelectParams {
   int max_slots;               // capacity of one histogram pass
   DeviceState* st;
   int max_nodes;
+  // wide columns (single GPU): the float thresholds k_scan_wide left per (level node, feature); null without wide columns
+  const int32_t* wide_of;      // [F] wide index, -1 for a byte column
+  const float* wide_thr_value; // [level nodes][f_count]
 };
+
+// The float threshold of candidate (level node j, local feature fl): a wide column's from k_scan_wide's side array, a
+// lossless byte column's from its packed threshold, NaN for a discretized one.
+__device__ __forceinline__ float candidate_thr_value(const SelectParams& p, int j, int fl, int32_t thr) {
+  const int fg = p.f_begin + fl;
+  if (p.wide_thr_value != nullptr && p.wide_of[fg] >= 0) return p.wide_thr_value[static_cast<size_t>(j) * p.f_count + fl];
+  return p.bucket_values != nullptr ? thr_value_of(thr, p.bucket_values + static_cast<size_t>(fg) * kMaxBins) : __builtin_nanf("");
+}
 
 __global__ void __launch_bounds__(256) k_select_local(SelectParams p) {
   // One warp per node: lane l scans features l, l+32, ... in increasing order with strict '>'
@@ -780,7 +804,7 @@ __global__ void __launch_bounds__(256) k_select_local(SelectParams p) {
             TieAlt a{};
             const int fg = p.f_begin + fl;
             a.feature = fg; a.thr = thr_bin_of(c.thr); a.n_pos = c.n_pos; a.cond_type = p.feature_type[fg];
-            a.thr_value = p.bucket_values != nullptr ? thr_value_of(c.thr, p.bucket_values + static_cast<size_t>(fg) * kMaxBins) : __builtin_nanf("");
+            a.thr_value = candidate_thr_value(p, j, fl, c.thr);
             if (a.cond_type == 1) {
               const uint32_t* m = p.cand_mask + (static_cast<size_t>(j) * p.f_count + fl) * 8;
               const int na = p.na_bin[fg];
@@ -896,8 +920,8 @@ __global__ void __launch_bounds__(256) k_select_global(SelectParams p) {
       if (nd->candidate) best = merge_shard_bests(p.shard_best, p.world, p.max_level_nodes, j);
       if (best.feature >= 0 && best.n_pos > 0 && best.n_pos < nd->n) {
         nd->feature = best.feature;
-        nd->thr_value = p.bucket_values != nullptr && best.cond_type == 0
-                            ? thr_value_of(best.thr, p.bucket_values + static_cast<size_t>(best.feature) * kMaxBins) : __builtin_nanf("");
+        // (a wide column's side-array entry is this rank's: wide columns are single GPU)
+        nd->thr_value = best.cond_type == 0 ? candidate_thr_value(p, j, best.feature - p.f_begin, best.thr) : __builtin_nanf("");
         best.thr = thr_bin_of(best.thr);
         nd->thr = best.thr;
         nd->cond_type = best.cond_type;
@@ -1025,6 +1049,8 @@ struct PartParams {
   unsigned long long* stats;  // [children of this level][3] fixed-point sums of g, h, g^2 (this rank's rows)
   int smem_children;          // capacity of the shared accumulators (children of this level)
   int smem_children_private;  // capacity with one accumulator copy per lane
+  const uint16_t* wide;       // k_partition_wide: the dataset's wide columns (ygg_dataset.d_wide / d_wide_of)
+  const int32_t* wide_of;
 };
 
 // Shared accumulators per child: cnt, g_lo, g_hi, h_lo, h_hi, g2_lo, g2_hi.
@@ -1074,8 +1100,9 @@ __device__ __forceinline__ PartNode make_part_node(const NodeRec* nodes, const N
 // node being split — g / h / q24 (128-bit loads), the relabel, the statistics of the smaller children and the
 // stable compaction of the rows histogrammed at the next level (block-wide exclusive scan; the list stays in ROW
 // ORDER, which k_hist relies on for conflict-free LDS.U8 reads of its bins tile).
-template <bool CAT>
-__global__ void __launch_bounds__(kPartThreads, 2) k_partition(PartParams p) {
+// WIDE (k_partition_wide, datasets with wide columns only): a split on a wide feature reads its uint16 code.
+template <bool CAT, bool WIDE>
+__device__ __forceinline__ void partition_impl(const PartParams& p) {
   extern __shared__ __align__(16) uint32_t smem[];
   __shared__ int s_warp_tot[kPartThreads / 32];
   __shared__ __align__(16) PartNode s_nodes[kPartMaxLevelNodes];
@@ -1123,7 +1150,9 @@ __global__ void __launch_bounds__(kPartThreads, 2) k_partition(PartParams p) {
         const uint4 a = *reinterpret_cast<const uint4*>(p.node_of_row + rh);
         nodew[0] = a.x; nodew[1] = a.y; nodew[2] = a.z; nodew[3] = a.w;
       }
-      // level-local node index (or -1) and the gathered split byte, packed: index << 8 | byte
+      // level-local node index (or -1) and the gathered split byte, packed: index << 8 | byte (WIDE: index << 16 | code;
+      // a level has at most 2^15 nodes)
+      constexpr int kBinBits = WIDE ? 16 : 8;
       int32_t lb[kPartRows];
       bool any = false;
 #pragma unroll
@@ -1134,7 +1163,10 @@ __global__ void __launch_bounds__(kPartThreads, 2) k_partition(PartParams p) {
           const int li = node - lv.first_node;
           const int feature = nodes_in_smem ? s_nodes[li].feature : p.nodes[node].feature;
           if (feature >= 0) {
-            lb[j] = (li << 8) | static_cast<int32_t>(p.bins[static_cast<int64_t>(feature) * p.n_pad + rh + j]);
+            const int wi = WIDE ? p.wide_of[feature] : -1;
+            const int32_t bin = wi >= 0 ? static_cast<int32_t>(p.wide[static_cast<int64_t>(wi) * p.n_pad + rh + j])
+                                        : static_cast<int32_t>(p.bins[static_cast<int64_t>(feature) * p.n_pad + rh + j]);
+            lb[j] = (li << kBinBits) | bin;
             any = true;
           }
         }
@@ -1161,8 +1193,8 @@ __global__ void __launch_bounds__(kPartThreads, 2) k_partition(PartParams p) {
             const int j = 4 * half + k;
             out_info[j] = 0u;
             if (lb[j] < 0) continue;
-            const int li = lb[j] >> 8;
-            const uint32_t bin = static_cast<uint32_t>(lb[j]) & 0xFFu;
+            const int li = lb[j] >> kBinBits;
+            const uint32_t bin = static_cast<uint32_t>(lb[j]) & ((1u << kBinBits) - 1u);
             const PartNode pn = nodes_in_smem ? s_nodes[li] : make_part_node<CAT>(p.nodes, p.nodes[lv.first_node + li]);
             // EvalConditionDiscretizedHigher (decision_tree.cc:724-743) / Contains (:766-812); NA is
             // already folded into na_bin.
@@ -1260,6 +1292,10 @@ __global__ void __launch_bounds__(kPartThreads, 2) k_partition(PartParams p) {
     }
   }
 }
+template <bool CAT>
+__global__ void __launch_bounds__(kPartThreads, 2) k_partition(PartParams p) { partition_impl<CAT, false>(p); }
+template <bool CAT>
+__global__ void __launch_bounds__(kPartThreads, 2) k_partition_wide(PartParams p) { partition_impl<CAT, true>(p); }
 
 // ---------------------------------------------------------------------------------------------
 // k_node_stats: fixed-point sums -> the doubles the reference stores, and the Newton leaf value.
@@ -1495,8 +1531,10 @@ __global__ void __launch_bounds__(1024) k_weight_sums_finish(WeightSumParams p) 
 // the node to the same side (twin columns); equal float scores and equal positive counts do not prove that.  Every
 // row walks from its leaf to the root; at each ancestor with recorded ties it knows on which side it went and
 // evaluates the alternatives' conditions: a disagreement disqualifies the alternative (n_pos = -1).
+// (`wide` / `wide_of`: the dataset's wide columns, null without them)
 __global__ void __launch_bounds__(256) k_verify_ties(NodeRec* nodes, const uint16_t* __restrict__ node_of_row,
-                                                     const uint8_t* __restrict__ bins, int64_t n, int64_t n_pad) {
+                                                     const uint8_t* __restrict__ bins, int64_t n, int64_t n_pad,
+                                                     const uint16_t* __restrict__ wide, const int32_t* __restrict__ wide_of) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n; r += stride) {
     int child = node_of_row[r];
@@ -1508,7 +1546,8 @@ __global__ void __launch_bounds__(256) k_verify_ties(NodeRec* nodes, const uint1
         for (int i = 0; i < min(tc, kMaxTieAlts); i++) {
           const TieAlt& a = nodes[node].tie[i];
           if (a.n_pos < 0) continue;
-          const uint32_t b = bins[static_cast<int64_t>(a.feature) * n_pad + r];
+          const int wi = wide_of != nullptr ? wide_of[a.feature] : -1;
+          const uint32_t b = wi >= 0 ? wide[static_cast<int64_t>(wi) * n_pad + r] : bins[static_cast<int64_t>(a.feature) * n_pad + r];
           const bool alt_pos = a.cond_type == 1 ? ((a.mask[b >> 5] >> (b & 31)) & 1u) != 0 : static_cast<int>(b) >= a.thr;
           if (alt_pos != went_pos) nodes[node].tie[i].n_pos = -1;
         }
@@ -1542,7 +1581,9 @@ __global__ void k_reset_loss(DeviceState* st) {
 
 // SplitExamplesInPlace as a standalone stable partition of a row-id list (single CTA per 2048-row
 // tile + decoupled offsets are overkill for a test seam: two-pass count/scatter with a global scan).
-__global__ void k_partition_count(const uint8_t* col, const uint32_t* rows, int64_t n, int thr,
+// (T: uint8_t for a byte column, uint16_t for a wide one)
+template <typename T>
+__global__ void k_partition_count(const T* col, const uint32_t* rows, int64_t n, int thr,
                                   uint32_t* block_pos_counts) {
   __shared__ uint32_t s[8];
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -1557,7 +1598,8 @@ __global__ void k_partition_count(const uint8_t* col, const uint32_t* rows, int6
   }
 }
 
-__global__ void k_partition_scatter(const uint8_t* col, const uint32_t* rows, int64_t n, int thr,
+template <typename T>
+__global__ void k_partition_scatter(const T* col, const uint32_t* rows, int64_t n, int thr,
                                     const uint32_t* block_pos_offsets, uint32_t total_pos,
                                     uint32_t* out) {
   __shared__ uint32_t s[8];

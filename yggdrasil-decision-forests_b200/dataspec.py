@@ -35,8 +35,22 @@ class DiscretizedColumn:
     bucket_values: Optional[np.ndarray] = None   # lossless columns: the value of every bucket (exact threshold rule)
     feature_type = _capi.FEATURE_DISCRETIZED_NUMERICAL
 
+    @property
+    def wide(self) -> bool:
+        """More buckets than a byte holds: a wide column (uint16 codes, _capi.Dataset.set_wide_column)."""
+        return self.num_bins > 256
+
     def encode(self, values) -> np.ndarray:
         return _capi.discretize_encode(np.asarray(values, dtype=np.float32), self.boundaries, self.na_bin)
+
+    def encode16(self, values) -> np.ndarray:
+        """uint16 codes by encode's rule (bucket = upper_bound(boundaries, x), NaN -> na_bin), for up to 65535 buckets."""
+        if self.num_bins > 65535:
+            raise ValueError(f"column {self.name!r}: {self.num_bins} buckets do not fit uint16 codes below 65535")
+        v = np.asarray(values, dtype=np.float32)
+        out = np.searchsorted(np.asarray(self.boundaries, dtype=np.float32), v, side="right").astype(np.uint16)
+        out[np.isnan(v)] = self.na_bin
+        return out
 
 
 @dataclasses.dataclass
@@ -179,7 +193,7 @@ def infer_column_lossless(name: str, values, max_rows: Optional[int] = None,
     # every row's value must have its own bucket: the distinct set comes from ALL rows, whatever `max_rows` says
     # about the statistics (a value outside the sample would otherwise be merged into a neighbour's bucket)
     distinct = np.unique(v[~np.isnan(v)])
-    if len(distinct) == 0 or len(distinct) > max_distinct:   # the engine's buckets are bytes
+    if len(distinct) == 0 or len(distinct) > max_distinct:   # byte buckets, or wide columns up to max_distinct values
         return None
     mean = float(present.astype(np.float64).mean()) if len(present) else float(distinct.astype(np.float64).mean())
     num_missing = int(np.isnan(v).sum())
@@ -200,8 +214,31 @@ def infer_column_lossless(name: str, values, max_rows: Optional[int] = None,
 
 
 def encode_features(cols: Dict[str, np.ndarray], columns: Sequence[DiscretizedColumn]) -> np.ndarray:
+    """[features, rows] bucket indices: uint8, or uint16 when a column has more than 256 buckets (wide columns)."""
     n = len(next(iter(cols.values())))
-    out = np.empty((len(columns), n), dtype=np.uint8)
+    wide = any(c.num_bins > 256 for c in columns)
+    out = np.empty((len(columns), n), dtype=np.uint16 if wide else np.uint8)
     for i, c in enumerate(columns):
-        out[i] = c.encode(cols[c.name])
+        out[i] = c.encode16(cols[c.name]) if c.num_bins > 256 else c.encode(cols[c.name])
     return out
+
+
+def device_dataset(bins: np.ndarray, columns: Sequence, device: int = 0) -> "_capi.Dataset":
+    """The device dataset of encode_features' output: byte columns as they are, wide columns (more than 256 buckets)
+    attached with their codes, bucket values and mean."""
+    wide = [i for i, c in enumerate(columns) if c.num_bins > 256]
+    byte_bins = np.zeros(bins.shape, np.uint8) if bins.dtype != np.uint8 else bins
+    if bins.dtype != np.uint8:
+        narrow = [i for i in range(len(columns)) if i not in set(wide)]
+        byte_bins[narrow] = bins[narrow]
+    num_bins = [1 if i in wide else c.num_bins for i, c in enumerate(columns)]
+    na_bin = [0 if i in wide else c.na_bin for i, c in enumerate(columns)]
+    ds = _capi.Dataset(byte_bins, num_bins, na_bin, device=device, feature_types=[c.feature_type for c in columns])
+    try:
+        for i in wide:
+            c = columns[i]
+            ds.set_wide_column(i, bins[i], c.num_bins, c.na_bin, c.bucket_values, c.mean)
+    except Exception:
+        ds.close()
+        raise
+    return ds

@@ -36,6 +36,7 @@ class GradientBoostedTreesLearner:
                  features: Optional[List[str]] = None,
                  weights: Optional[str] = None,
                  discretize_numerical_columns: bool = False,
+                 max_exact_numerical_values: int = 255,
                  num_discretized_numerical_bins: int = 255,
                  max_num_scanned_rows_to_compute_statistics: Optional[int] = None,
                  min_vocab_frequency: int = 5,
@@ -88,9 +89,19 @@ class GradientBoostedTreesLearner:
         # discretize_numerical_columns=False (the reference's default) asks for the EXACT numerical splitter.  This engine
         # is the bucketised split finder, but with one bucket per distinct value it examines exactly the exact splitter's
         # candidate cuts (dataspec.infer_column_lossless; default runs of the reference replayed that way in
-        # tests/test_reference_replay.py), so the option is honoured for columns with at most 255 distinct values and
-        # refused — not approximated — for the others (_build_dataset).
+        # tests/test_reference_replay.py), so the option is honoured for columns with at most 255 distinct values (byte
+        # buckets), for wider ones up to max_exact_numerical_values (wide columns), and refused — not approximated — for
+        # the others (_build_dataset).
         self.discretize_numerical_columns = bool(discretize_numerical_columns)
+        # The largest numerical column (distinct values) the exact splitter takes.  Columns of up to 255 values use byte
+        # buckets; wider ones, up to this limit, become wide columns (uint16 buckets, DESIGN.md §20), whose histogram
+        # memory grows with their buckets: a resource bound, like max_vocab_count.
+        if isinstance(max_exact_numerical_values, bool) or not isinstance(max_exact_numerical_values, (int, np.integer)):
+            raise TypeError("max_exact_numerical_values must be an integer")
+        if not 255 <= int(max_exact_numerical_values) <= 65535:
+            raise ValueError(f"max_exact_numerical_values={max_exact_numerical_values} outside [255, 65535] "
+                             "(wide columns hold at most 65535 buckets)")
+        self.max_exact_numerical_values = int(max_exact_numerical_values)
         if not 0.0 <= validation_ratio <= 1.0:
             raise ValueError("The validation set ratio should be in [0,1].")
         if early_stopping not in _EARLY_STOPPING:
@@ -173,12 +184,14 @@ class GradientBoostedTreesLearner:
         if not self.discretize_numerical_columns:   # checked before anything is created on the device
             for name in names:
                 if cols[name].dtype.kind in "fiub":
-                    lossless[name] = ds_lib.infer_column_lossless(name, cols[name], self.max_rows_stats)
-                    if lossless[name] is None:
+                    limit = self.max_exact_numerical_values
+                    lossless[name] = ds_lib.infer_column_lossless(name, cols[name], self.max_rows_stats, max_distinct=limit)
+                    if lossless[name] is None or lossless[name].num_bins > 65535:
                         raise NotImplementedError(
-                            f'column "{name}" has more than 255 distinct values: the exact numerical splitter is only '
-                            "reproduced for columns that fit one bucket per value; pass discretize_numerical_columns=True "
-                            "for the reference's 255-bin discretisation")
+                            f'column "{name}" has more than {limit} distinct values: the exact numerical splitter is only '
+                            "reproduced for columns that fit one bucket per value, up to max_exact_numerical_values "
+                            f"(= {limit}; at most 65535 buckets with the mean of the missing values); raise it, or pass "
+                            "discretize_numerical_columns=True for the reference's 255-bin discretisation")
         builder = _capi.DatasetBuilder(n, len(names), device=self.device)
         columns = [None] * len(names)
         pending = []
@@ -195,7 +208,10 @@ class GradientBoostedTreesLearner:
                     raise NotImplementedError(f'column "{name}" has unsupported dtype {v.dtype}')
                 elif not self.discretize_numerical_columns:
                     c = lossless[name]
-                    builder.add_bins(f, c.encode(v), c.num_bins, c.na_bin, _capi.FEATURE_DISCRETIZED_NUMERICAL)
+                    if c.wide:   # attached after finish(); the byte column is a placeholder
+                        builder.add_bins(f, np.zeros(n, np.uint8), 1, 0, _capi.FEATURE_DISCRETIZED_NUMERICAL)
+                    else:
+                        builder.add_bins(f, c.encode(v), c.num_bins, c.na_bin, _capi.FEATURE_DISCRETIZED_NUMERICAL)
                     columns[f] = c
                 elif self.num_discretized_numerical_bins < 4:
                     # the GPU rule needs >= 4 bins (two are reserved for the special values); host rule below
@@ -215,7 +231,14 @@ class GradientBoostedTreesLearner:
                                                       num_missing=int(missing), num_values=n)
             dataset = builder.finish()
             for f, c in enumerate(columns):   # exact numerical splitter: thresholds between the values present in a node
-                if getattr(c, "bucket_values", None) is not None and len(c.bucket_values) <= 255:
+                if getattr(c, "bucket_values", None) is None:
+                    continue
+                if c.wide:
+                    dataset.set_wide_column(f, c.encode16(cols[c.name]), c.num_bins, c.na_bin, c.bucket_values, c.mean)
+                elif len(c.bucket_values) <= 255 or c.num_missing == 0:
+                    # (256 buckets without a missing value: 256 distinct values, which max_exact_numerical_values >= 256
+                    # lets through; the byte path carries them with the exact rule.  255 values + the mean keep the
+                    # discretized rule, as before.)
                     dataset.set_bucket_values(f, c.bucket_values, c.mean)
         except Exception:
             builder.close()
@@ -281,8 +304,7 @@ class GradientBoostedTreesLearner:
             if valid is not None:
                 vcols = ds_lib.as_columns(valid)
                 vbins = ds_lib.encode_features(vcols, spec.columns)
-                valid_ds = _capi.Dataset(vbins, [c.num_bins for c in spec.columns], [c.na_bin for c in spec.columns],
-                                         device=self.device, feature_types=[c.feature_type for c in spec.columns])
+                valid_ds = ds_lib.device_dataset(vbins, spec.columns, device=self.device)
                 valid_labels = self._labels(vcols, spec)
                 valid_weights = self._weights(vcols)
             elif self.validation_ratio > 0.0:

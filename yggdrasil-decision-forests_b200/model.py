@@ -55,7 +55,8 @@ class GradientBoostedTreesModel:
                 nd = node[idx]
                 f = t["feature"][nd]
                 b = bins[f, idx].astype(np.int64)
-                in_set = (t["cat_mask"][nd, b >> 5] >> (b & 31).astype(np.uint32)) & 1
+                # (the mask is only read for categorical conditions, whose bins are bytes; a wide column's code may not be)
+                in_set = (t["cat_mask"][nd, np.minimum(b >> 5, 7)] >> (b & 31).astype(np.uint32)) & 1
                 go_pos = np.where(t["condition_type"][nd] == 1, in_set != 0, b >= t["threshold_bin"][nd])
                 node[idx] = np.where(go_pos, t["pos_child"][nd], t["neg_child"][nd])
                 active = t["feature"][node] >= 0
