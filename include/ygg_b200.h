@@ -115,7 +115,8 @@ enum ygg_early_stopping {
  * Mirrors proto::Node + proto::NodeCondition (model/decision_tree/decision_tree.proto). */
 enum ygg_feature_type {
   YGG_FEATURE_DISCRETIZED_NUMERICAL = 0, /* condition: bin >= threshold_bin */
-  YGG_FEATURE_CATEGORICAL = 1            /* condition: category in cat_mask (CART, < 300 values) */
+  YGG_FEATURE_CATEGORICAL = 1            /* condition: category in cat_mask (CART); a wide categorical column's set
+                                            is read with ygg_gbt_get_category_set */
 };
 
 typedef struct ygg_node {
@@ -167,8 +168,9 @@ int ygg_device_count(void);
  * byte layout: value = integerised category (0 = out-of-dictionary), num_bins[f] =
  * number_of_unique_values <= 256, na_bin[f] = most_frequent_value (the NA replacement,
  * training.cc:3262-3314); they are split with the CART rule (buckets sorted by label mean /
- * hessian priority, then scanned).  Columns with >= 300 values (random-mask algorithm,
- * decision_tree.proto:576) do not fit one byte and are rejected.
+ * hessian priority, then scanned).  Columns with 257..65535 categories are wide categorical columns
+ * (ygg_dataset_set_wide_categorical_column), also split with CART: the engine has no random-mask algorithm
+ * (decision_tree.proto:573-576), which is the learner's business (categorical_arity_limit_for_random).
  *  device      : CUDA ordinal this handle lives on (one process per GPU).
  */
 int ygg_dataset_create(ygg_dataset** out, int64_t n_rows, int32_t n_features,
@@ -195,6 +197,13 @@ int ygg_dataset_set_bucket_values(ygg_dataset* ds, int32_t feature, const float*
  * and validation / prediction datasets must have the same wide features and buckets. */
 int ygg_dataset_set_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
                                 const float* values, float na_replacement);
+/* Wide categorical column (DESIGN.md §21): a feature already set to YGG_FEATURE_CATEGORICAL with num_bins = 257..65535
+ * categories (number_of_unique_values), codes[r] < num_bins the category of row r (missing values already folded into
+ * na_bin = most_frequent_value).  Split with CART like a byte categorical column; the positive set of such a split is
+ * read with ygg_gbt_get_category_set (its ygg_node.cat_mask is zero).  Same rules as ygg_dataset_set_wide_column: before
+ * ygg_gbt_create, single GPU, validation / prediction datasets with the same wide columns. */
+int ygg_dataset_set_wide_categorical_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins,
+                                            int32_t na_bin);
 /* Read-back of a wide column: codes[n_rows], and (may be NULL) its num_bins / na_bin. */
 int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t* codes, int32_t* num_bins, int32_t* na_bin);
 int ygg_dataset_destroy(ygg_dataset* ds);
@@ -341,6 +350,12 @@ int ygg_gbt_set_tie_rng_position(ygg_gbt* h, uint64_t words);
 /* Copies tree `iter` (pre-order: node, neg subtree, pos subtree).  *n_nodes receives the node
  * count; fails with INVALID_ARGUMENT if capacity is too small. */
 int ygg_gbt_get_tree(ygg_gbt* h, int32_t iter, ygg_node* out, int32_t capacity, int32_t* n_nodes);
+/* The positive set of categorical split `node` (pre-order index, as in ygg_gbt_get_tree) of tree `iter` (-1: the tree
+ * the last ygg_tree_train_on_gradients call returned): bit c of
+ * words[c / 32] set => category c goes to the positive child.  *n_words = ceil(num_bins / 32) for a wide categorical
+ * column, 8 (cat_mask) for a byte one; fails with INVALID_ARGUMENT if capacity is smaller or the node is not a
+ * categorical split. */
+int ygg_gbt_get_category_set(ygg_gbt* h, int32_t iter, int32_t node, uint32_t* words, int32_t capacity, int32_t* n_words);
 /* Training loss / secondary metric after iteration `iter` (loss->Loss,
  * gradient_boosted_trees.cc:1575-1580): binomial => (2x mean log-loss, accuracy);
  * squared error => (rmse, rmse). */
@@ -358,7 +373,8 @@ int ygg_gbt_set_predictions(ygg_gbt* h, const float* pred, int64_t n);
 
 /* decision_tree::Train seam (learner/decision_tree/training.h:1012-1021): grows ONE regression
  * tree on caller-provided per-example gradients / hessians (host pointers) with the handle's
- * tree hyper-parameters; does not touch the boosting state. */
+ * tree hyper-parameters; does not touch the boosting state.  The positive sets of its splits on wide categorical
+ * columns are read with ygg_gbt_get_category_set(h, -1, ...). */
 int ygg_tree_train_on_gradients(ygg_gbt* h, const float* gradients, const float* hessians,
                                 ygg_node* out, int32_t capacity, int32_t* n_nodes);
 

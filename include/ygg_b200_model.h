@@ -41,6 +41,10 @@ typedef struct ygg_model_desc {
   const int32_t* feature_num_values; /* [num_features]: CategoricalSpec.number_of_unique_values of a categorical
                                         feature (sizes Condition.ContainsBitmap); may be NULL without
                                         categorical features */
+  const int64_t* node_set_offset;  /* [tree_offsets[num_trees]] or NULL: for a categorical split on a column with more
+                                      than 256 values, the offset of its positive set (ceil(num_values / 32) words) in
+                                      cat_set_words; -1 for the other nodes, whose set is cat_mask */
+  const uint32_t* cat_set_words;
 } ygg_model_desc;
 
 int ygg_model_write_ydf(const ygg_model_desc* desc);

@@ -78,6 +78,7 @@ EXPORTS = [
     "ygg_gbt_best_split_window_bytes", "ygg_gbt_set_best_split_window", "ygg_comm_window_create",
     "ygg_comm_unique_id", "ygg_comm_create", "ygg_comm_destroy", "ygg_comm_allreduce", "ygg_comm_allgather", "ygg_comm_reducescatter",
     "ygg_dataset_set_wide_column", "ygg_dataset_get_wide_column", "ygg_debug_wide_histogram",
+    "ygg_dataset_set_wide_categorical_column", "ygg_gbt_get_category_set",
 ]
 
 
@@ -158,6 +159,18 @@ class Dataset:
         check(lib().ygg_dataset_set_wide_column(self.handle, C.c_int32(int(feature)), ptr(c, C.c_uint16), C.c_int64(len(c)),
                                                 C.c_int32(int(num_bins)), C.c_int32(int(na_bin)), ptr(v, C.c_float),
                                                 C.c_float(float(np.float32(na_replacement)))))
+        self.num_bins = self.num_bins.copy()
+        self.na_bin = self.na_bin.copy()
+        self.num_bins[feature], self.na_bin[feature] = 1, 0   # the byte column is a one-bucket filler
+        self.wide = dict(getattr(self, "wide", {}))
+        self.wide[int(feature)] = (int(num_bins), int(na_bin))
+
+    def set_wide_categorical_column(self, feature, codes, num_bins, na_bin):
+        """Wide categorical column (257..65535 categories): codes[r] = the uint16 category of row r, na_bin = the
+        most_frequent_value missing values were folded into.  The feature must already be FEATURE_CATEGORICAL."""
+        c = np.ascontiguousarray(codes, dtype=np.uint16)
+        check(lib().ygg_dataset_set_wide_categorical_column(self.handle, C.c_int32(int(feature)), ptr(c, C.c_uint16),
+                                                            C.c_int64(len(c)), C.c_int32(int(num_bins)), C.c_int32(int(na_bin))))
         self.num_bins = self.num_bins.copy()
         self.na_bin = self.na_bin.copy()
         self.num_bins[feature], self.na_bin[feature] = 1, 0   # the byte column is a one-bucket filler
@@ -557,6 +570,26 @@ class Gbt:
         check(lib().ygg_gbt_get_tree(self.handle, C.c_int32(it), out.ctypes.data_as(C.c_void_p),
                                      C.c_int32(cap), C.byref(n)))
         return out[:n.value].copy()
+
+    def get_category_sets(self, it, tree=None):
+        """{pre-order node index: uint32 words} of the splits of tree `it` on wide categorical columns (bit c of
+        words[c // 32] set: category c is positive); `it` = -1: the tree of the last train_tree_on_gradients call.
+        `tree`: that tree, if already fetched (required for -1)."""
+        wide = getattr(self.dataset, "wide", {})
+        if not wide:
+            return {}
+        t = self.get_tree(it) if tree is None else tree
+        out = {}
+        for i in np.flatnonzero((t["condition_type"] == FEATURE_CATEGORICAL) & (t["feature"] >= 0)):
+            f = int(t["feature"][i])
+            if f not in wide:
+                continue
+            words = np.zeros((wide[f][0] + 31) // 32, np.uint32)
+            n = C.c_int32()
+            check(lib().ygg_gbt_get_category_set(self.handle, C.c_int32(it), C.c_int32(int(i)), ptr(words, C.c_uint32),
+                                                 C.c_int32(len(words)), C.byref(n)))
+            out[int(i)] = words
+        return out
 
     def train_loss(self, it):
         a, b = C.c_float(), C.c_float()

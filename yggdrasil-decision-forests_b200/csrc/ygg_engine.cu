@@ -178,6 +178,19 @@ struct ygg_gbt {
   float* d_wide_thr = nullptr;       // [split-level nodes][f_scan]
   int32_t* d_wide_feature = nullptr; // [wide features]
   int32_t* d_wide_bins = nullptr;
+  // wide categorical columns (DESIGN.md §21): per-feature tables, the level's positive sets [split-level nodes][n_wide]
+  // [set_words], the scan's sort scratch, and the positive-set pool [tree capacity + 1][max_nodes][set_words] (the last
+  // tree is d_nodes_scratch's)
+  int set_words = 0;
+  int64_t sort_total = 0;            // sort scratch entries per CTA: sort_pad(B_w) summed over the wide categorical columns
+  int64_t* d_sort_off = nullptr;     // [wide features] a column's block of the scratch
+  int32_t* d_wide_cat = nullptr;
+  int32_t* d_wide_na_bin = nullptr;
+  uint32_t* d_wide_set = nullptr;
+  double* d_sort_key = nullptr;
+  int32_t* d_sort_idx = nullptr;
+  uint32_t* d_sets = nullptr;
+  bool scratch_tree = false;         // d_nodes_scratch holds the tree of the last ygg_tree_train_on_gradients call
   ShardBest* d_shard_best = nullptr;
   TieRec* d_ties = nullptr;        // [max level nodes] ties of the level being selected (single GPU)
   // stochastic gradient boosting (cfg.subsample < 1): this iteration's sample, drawn on the host from the learner's engine
@@ -626,6 +639,10 @@ int allocate_wide_buffers(ygg_gbt* h) {
   }
   dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins);
   h->d_wide_thr = nullptr; h->d_wide_feature = nullptr; h->d_wide_bins = nullptr;
+  dev_free(h->d_wide_cat); dev_free(h->d_wide_na_bin); dev_free(h->d_wide_set); dev_free(h->d_sort_key); dev_free(h->d_sort_idx);
+  h->d_wide_cat = nullptr; h->d_wide_na_bin = nullptr; h->d_wide_set = nullptr; h->d_sort_key = nullptr; h->d_sort_idx = nullptr;
+  dev_free(h->d_sort_off); h->d_sort_off = nullptr;
+  h->sort_total = 0;
   h->wide_total = 0;
   h->wide_slots = 0;
   if (ds->n_wide() == 0 || h->num_levels == 0) return YGG_OK;
@@ -656,7 +673,43 @@ int allocate_wide_buffers(ygg_gbt* h) {
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_bins, ds->n_wide()));
   YGG_CUDA(cudaMemcpy(h->d_wide_feature, ds->wide_feature.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
   YGG_CUDA(cudaMemcpy(h->d_wide_bins, ds->wide_bins.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+  if (h->set_words > 0) {
+    // wide categorical columns: (nodes x n_wide x set_words) x 4 B of positive sets, and (slots x sum of sort_pad(B_w)) x 12 B
+    // of sort scratch (sort_pad(B) = the power of two >= B, per column)
+    std::vector<int64_t> sort_off(ds->n_wide(), 0);
+    for (int w = 0; w < ds->n_wide(); w++) {
+      sort_off[w] = h->sort_total;
+      if (ds->wide_cat[w]) h->sort_total += sort_pad(ds->wide_bins[w]);
+    }
+    const size_t scratch = static_cast<size_t>(h->wide_slots) * h->sort_total;
+    if (dev_alloc(&h->d_wide_set, nodes * ds->n_wide() * h->set_words) != YGG_OK || dev_alloc(&h->d_sort_key, scratch) != YGG_OK ||
+        dev_alloc(&h->d_sort_idx, scratch) != YGG_OK) {
+      (void)cudaGetLastError();
+      return set_error(YGG_ERR_CUDA, "wide categorical columns: %.2f GB of positive sets and sort scratch could not be allocated; "
+                       "lower max_depth or the categories of the wide columns",
+                       (static_cast<double>(nodes) * ds->n_wide() * h->set_words * 4 + static_cast<double>(scratch) * 12) / 1e9);
+    }
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_cat, ds->n_wide()));
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_na_bin, ds->n_wide()));
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_sort_off, ds->n_wide()));
+    YGG_CUDA(cudaMemcpy(h->d_sort_off, sort_off.data(), sizeof(int64_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+    YGG_CUDA(cudaMemcpy(h->d_wide_cat, ds->wide_cat.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+    YGG_CUDA(cudaMemcpy(h->d_wide_na_bin, ds->wide_na_bin.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+  }
   return YGG_OK;
+}
+
+// Nodes per tree of the positive-set pool: only the split levels' nodes can split, and the ids of level l are below
+// 2^(l+1) - 1, so every split node's id is below 2^(max_depth-1) - 1 = max_nodes / 2.
+int pool_nodes(const ygg_gbt* h) { return std::max(1, h->max_nodes >> 1); }
+
+// The positive-set pool entry of tree `nodes` (one of d_nodes_all's trees, or d_nodes_scratch); null without wide
+// categorical columns.
+uint32_t* sets_of(ygg_gbt* h, const NodeRec* nodes) {
+  if (h->d_sets == nullptr) return nullptr;
+  const size_t tree = nodes == h->d_nodes_scratch ? static_cast<size_t>(h->tree_capacity)
+                                                   : static_cast<size_t>(nodes - h->d_nodes_all) / h->max_nodes;
+  return h->d_sets + tree * pool_nodes(h) * h->set_words;
 }
 
 // The wide columns' histogram phase of a level: zeroes the planes of `slots` slots and accumulates the level's active
@@ -967,11 +1020,20 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
         wp.node_sum = h->d_wnode_sum[par]; wp.node_cnt = h->d_wnode_cnt[par]; wp.node_hsum = h->d_wnode_hsum[par];
         wp.pnode_sum = h->d_wnode_sum[par ^ 1]; wp.pnode_cnt = h->d_wnode_cnt[par ^ 1]; wp.pnode_hsum = h->d_wnode_hsum[par ^ 1];
         wp.thr_value = h->d_wide_thr;
+        wp.wide_cat = h->d_wide_cat; wp.n_wide = ds->n_wide(); wp.set_words = h->set_words; wp.set_out = h->d_wide_set;
+        wp.sort_key = h->d_sort_key; wp.sort_idx = h->d_sort_idx; wp.sort_off = h->d_sort_off; wp.sort_total = h->sort_total;
         const dim3 wgrid(level_slot_bound(h, l), ds->n_wide());
         if (hist_hess(h) || use_hess(h)) k_scan_wide<true><<<wgrid, 256, 0, h->stream>>>(wp);
         else k_scan_wide<false><<<wgrid, 256, 0, h->stream>>>(wp);
         h->launches_total++;
         YGG_RETURN_IF_ERROR(check_launch("k_scan_wide"));
+        if (h->set_words > 0) {
+          ProfScope psc(h, "scan_wide_cat");
+          if (hist_hess(h) || use_hess(h)) k_scan_wide_cat<true><<<wgrid, 256, 0, h->stream>>>(wp);
+          else k_scan_wide_cat<false><<<wgrid, 256, 0, h->stream>>>(wp);
+          h->launches_total++;
+          YGG_RETURN_IF_ERROR(check_launch("k_scan_wide_cat"));
+        }
       }
     }
     {
@@ -991,6 +1053,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       sel.max_slots = (l + 1 < h->num_levels) ? level_slot_bound(h, l + 1) : 0x7fffffff;
       sel.st = h->d_st; sel.max_nodes = h->max_nodes;
       sel.wide_of = h->wide_total > 0 ? ds->d_wide_of : nullptr; sel.wide_thr_value = h->wide_total > 0 ? h->d_wide_thr : nullptr;
+      sel.wide_set = h->d_wide_set; sel.wide_na_bin = h->d_wide_na_bin; sel.n_wide = ds->n_wide(); sel.set_words = h->set_words;
       const int threads = 256, blocks = (level_nodes_bound + (threads / 32) - 1) / (threads / 32);
       k_select_local<<<blocks, threads, 0, h->stream>>>(sel);
       h->launches_total++;
@@ -1011,6 +1074,12 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       k_select_global<<<1, 256, 0, h->stream>>>(sel);
       h->launches_total++;
       YGG_RETURN_IF_ERROR(check_launch("k_select_global"));
+      if (h->d_wide_set != nullptr) {
+        k_store_sets<<<level_nodes_bound, 256, 0, h->stream>>>(nodes, h->d_levels, l, ds->d_wide_of, h->d_wide_set, ds->n_wide(),
+                                                               h->set_words, sets_of(h, nodes));
+        h->launches_total++;
+        YGG_RETURN_IF_ERROR(check_launch("k_store_sets"));
+      }
     }
     // children statistics go to the stats tail of the NEXT level's buffer layout
     const int children_bound = 2 << l;
@@ -1041,7 +1110,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
                                        [](int32_t t) { return t == YGG_FEATURE_CATEGORICAL; });
       const int pgrid = (h->n_blocks + per_cta - 1) / per_cta;
       if (ds->n_wide() > 0) {   // the byte-only instantiations stay as they are for datasets without wide columns
-        pp.wide = ds->d_wide; pp.wide_of = ds->d_wide_of;
+        pp.wide = ds->d_wide; pp.wide_of = ds->d_wide_of; pp.sets = sets_of(h, nodes); pp.set_words = h->set_words;
         if (any_cat) k_partition_wide<true><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
         else k_partition_wide<false><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
       } else if (any_cat) {
@@ -1207,7 +1276,8 @@ __device__ __forceinline__ uint32_t row_bin(const uint8_t* __restrict__ bins, co
 template <int LOSS>
 __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
                                                       const int32_t* __restrict__ wide_of, int64_t n, int64_t n_pad,
-                                                      const NodeRec* __restrict__ tree, float* __restrict__ pred,
+                                                      const NodeRec* __restrict__ tree, const uint32_t* __restrict__ sets,
+                                                      int set_words, float* __restrict__ pred,
                                                       const uint8_t* __restrict__ label_u8,
                                                       const float* __restrict__ label_f32, LossRec* out, LossPartials* partials,
                                                       const float* __restrict__ weight, float correct_scale) {
@@ -1220,8 +1290,8 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
       const int f = tree[node].feature;
       if (f < 0) break;
       const uint32_t b = row_bin(bins, wide, wide_of, n_pad, f, r);
-      const bool pos = tree[node].cond_type == 1 ? ((tree[node].mask[b >> 5] >> (b & 31)) & 1u) != 0
-                                                 : static_cast<int>(b) >= tree[node].thr;
+      const bool wide_split = wide_of != nullptr && wide_of[f] >= 0;
+      const bool pos = split_goes_pos(tree[node], b, wide_split, sets + static_cast<size_t>(node) * set_words);
       node = pos ? tree[node].pos_child : tree[node].neg_child;
     }
     const float p = pred[r] + tree[node].leaf_value;
@@ -1262,7 +1332,8 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
 // reached in every tree of the row's class plane.  One thread per row, trees in order (float sums in the reference's order).
 __global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
                                                 const int32_t* __restrict__ wide_of, int64_t n, int64_t n_pad, const NodeRec* __restrict__ trees,
-                                                int max_nodes, int n_trees, int K, float initial, float* __restrict__ out /*[K][n]*/) {
+                                                const uint32_t* __restrict__ sets, int set_words, int pool_nodes, int max_nodes, int n_trees, int K,
+                                                float initial, float* __restrict__ out /*[K][n]*/) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n; r += stride) {
     for (int k = 0; k < K; k++) {
@@ -1274,8 +1345,9 @@ __global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bin
           const int f = tree[node].feature;
           if (f < 0) break;
           const uint32_t b = row_bin(bins, wide, wide_of, n_pad, f, r);
-          const bool pos = tree[node].cond_type == 1 ? ((tree[node].mask[b >> 5] >> (b & 31)) & 1u) != 0
-                                                     : static_cast<int>(b) >= tree[node].thr;
+          const bool wide_split = wide_of != nullptr && wide_of[f] >= 0;
+          const bool pos = split_goes_pos(tree[node], b, wide_split,
+                                          sets + (static_cast<size_t>(t) * pool_nodes + node) * set_words);
           node = pos ? tree[node].pos_child : tree[node].neg_child;
         }
         acc += tree[node].leaf_value;
@@ -1293,7 +1365,7 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
   const int64_t nv = h->vds->n;
   const int grid = static_cast<int>(std::min<int64_t>((nv + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 8));
   if (is_multinomial(h)) {
-    k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, h->d_vpred + static_cast<int64_t>(plane) * nv,
+    k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred + static_cast<int64_t>(plane) * nv,
                                                    nullptr, nullptr, nullptr, nullptr, nullptr, 0.f);
     h->launches_total++;
     YGG_RETURN_IF_ERROR(check_launch("k_valid_update"));
@@ -1310,11 +1382,11 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
     return YGG_OK;
   }
   if (h->cfg.loss == YGG_LOSS_BINOMIAL_LOG_LIKELIHOOD)
-    k_valid_update<0><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, h->d_vpred, h->d_vlabel_u8,
+    k_valid_update<0><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
                                                    h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
                                                    h->d_vweight, h->v_correct_scale);
   else
-    k_valid_update<1><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, h->d_vpred, h->d_vlabel_u8,
+    k_valid_update<1><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
                                                    h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
                                                    h->d_vweight, h->v_correct_scale);
   h->launches_total++;
@@ -1700,6 +1772,14 @@ void preorder(const std::vector<NodeRec>& nodes, int idx, std::vector<ygg_node>*
   (*out)[my] = o;
 }
 
+// The node ids of preorder's output, in its order.
+void preorder_ids(const std::vector<NodeRec>& nodes, int idx, std::vector<int>* out) {
+  out->push_back(idx);
+  if (nodes[idx].feature < 0) return;
+  preorder_ids(nodes, nodes[idx].neg_child, out);
+  preorder_ids(nodes, nodes[idx].pos_child, out);
+}
+
 // resolve: the tree is not one of the handle's own (ygg_tree_train_on_gradients): break its ties here, with the
 // handle's stream where it stands.
 int fetch_tree(ygg_gbt* h, const NodeRec* d_nodes, std::vector<ygg_node>* out, bool resolve = false) {
@@ -1709,7 +1789,11 @@ int fetch_tree(ygg_gbt* h, const NodeRec* d_nodes, std::vector<ygg_node>* out, b
   YGG_CUDA(cudaStreamSynchronize(h->stream));
   if (resolve && h->cfg.candidate_shuffle != 0) {
     ensure_tie_rng(h);
-    resolve_tree_on_host(h, nodes.data());
+    if (resolve_tree_on_host(h, nodes.data())) {   // the device table follows (ygg_gbt_get_category_set reads it)
+      YGG_CUDA(cudaMemcpyAsync(const_cast<NodeRec*>(d_nodes), nodes.data(), sizeof(NodeRec) * h->max_nodes, cudaMemcpyHostToDevice,
+                               h->stream));
+      YGG_CUDA(cudaStreamSynchronize(h->stream));
+    }
   }
   out->clear();
   preorder(nodes, 0, out);
@@ -1863,26 +1947,20 @@ int ensure_exact_arrays(ygg_dataset* ds) {
 }
 }  // namespace
 
-int ygg_dataset_set_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
-                                const float* values, float na_replacement) {
-  // the checks that need no dataset first (they hold without a device too), then those against the dataset
-  if (!codes || !values) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
-  if (num_bins < kMaxBins + 1 || num_bins > 65535)
-    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: num_bins=%d outside [257, 65535] (fewer fit the byte columns)", feature, num_bins);
-  if (na_bin < 0 || na_bin >= num_bins) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: na_bin=%d outside [0, num_bins)", feature, na_bin);
-  if (n < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "negative row count %lld", static_cast<long long>(n));
-  for (int i = 0; i < num_bins; i++)
-    if (!std::isfinite(values[i]) || (i > 0 && !(values[i] > values[i - 1])))
-      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: bucket values must be finite and strictly ascending", feature);
-  for (int64_t r = 0; r < n; r++)
-    if (codes[r] >= num_bins)
-      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: code %u of row %lld >= num_bins=%d", feature, codes[r], static_cast<long long>(r), num_bins);
+namespace {
+// The dataset checks and the upload shared by the wide numerical and the wide categorical columns (`values` null:
+// categorical; its bucket values are zeros).
+int attach_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
+                       const float* values, float na_replacement) {
+  const bool categorical = values == nullptr;
   if (!ds) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
   if (ds->handles > 0)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "wide columns are set before ygg_gbt_create: %d handle(s) already use this dataset", ds->handles);
-  if (ds->feature_type[feature] != YGG_FEATURE_DISCRETIZED_NUMERICAL)
-    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is categorical: wide columns are numerical", feature);
+  if (!categorical && ds->feature_type[feature] != YGG_FEATURE_DISCRETIZED_NUMERICAL)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is categorical: use ygg_dataset_set_wide_categorical_column", feature);
+  if (categorical && ds->feature_type[feature] != YGG_FEATURE_CATEGORICAL)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is not YGG_FEATURE_CATEGORICAL (ygg_dataset_set_feature_types first)", feature);
   if (!ds->wide_of.empty() && ds->wide_of[feature] >= 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is already a wide column", feature);
   if (n != ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "%lld codes for a dataset of %lld rows", static_cast<long long>(n), static_cast<long long>(ds->n));
   YGG_RETURN_IF_ERROR(require_device());
@@ -1911,15 +1989,49 @@ int ygg_dataset_set_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t
   ds->wide_feature.push_back(feature);
   ds->wide_bins.push_back(num_bins);
   ds->wide_na_bin.push_back(na_bin);
+  ds->wide_cat.push_back(categorical ? 1 : 0);
   ds->wide_na_replacement.push_back(na_replacement);
-  ds->wide_values.insert(ds->wide_values.end(), values, values + num_bins);
+  if (categorical) ds->wide_values.insert(ds->wide_values.end(), static_cast<size_t>(num_bins), 0.f);
+  else ds->wide_values.insert(ds->wide_values.end(), values, values + num_bins);
   ds->wide_off.push_back(ds->wide_off.back() + num_bins);
   YGG_RETURN_IF_ERROR(upload_wide_meta(ds));
+  if (categorical) return YGG_OK;
   YGG_RETURN_IF_ERROR(ensure_exact_arrays(ds));
   const int32_t zero = 0;
   YGG_CUDA(cudaMemcpy(ds->d_exact_rule + feature, &zero, sizeof(zero), cudaMemcpyHostToDevice));
   YGG_CUDA(cudaMemcpy(ds->d_na_replacement + feature, &na_replacement, sizeof(float), cudaMemcpyHostToDevice));
   return YGG_OK;
+}
+
+// The argument checks that need no dataset (they hold without a device too).
+int check_wide_codes(int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin) {
+  if (!codes) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (num_bins < kMaxBins + 1 || num_bins > 65535)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: num_bins=%d outside [257, 65535] (fewer fit the byte columns)", feature, num_bins);
+  if (na_bin < 0 || na_bin >= num_bins) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: na_bin=%d outside [0, num_bins)", feature, na_bin);
+  if (n < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "negative row count %lld", static_cast<long long>(n));
+  for (int64_t r = 0; r < n; r++)
+    if (codes[r] >= num_bins)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: code %u of row %lld >= num_bins=%d", feature, codes[r], static_cast<long long>(r), num_bins);
+  return YGG_OK;
+}
+}  // namespace
+
+int ygg_dataset_set_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
+                                const float* values, float na_replacement) {
+  // the checks that need no dataset first (they hold without a device too), then those against the dataset
+  if (!values) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  YGG_RETURN_IF_ERROR(check_wide_codes(feature, codes, n, num_bins, na_bin));
+  for (int i = 0; i < num_bins; i++)
+    if (!std::isfinite(values[i]) || (i > 0 && !(values[i] > values[i - 1])))
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: bucket values must be finite and strictly ascending", feature);
+  return attach_wide_column(ds, feature, codes, n, num_bins, na_bin, values, na_replacement);
+}
+
+int ygg_dataset_set_wide_categorical_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins,
+                                            int32_t na_bin) {
+  YGG_RETURN_IF_ERROR(check_wide_codes(feature, codes, n, num_bins, na_bin));
+  return attach_wide_column(ds, feature, codes, n, num_bins, na_bin, nullptr, 0.f);
 }
 
 int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t* codes, int32_t* num_bins, int32_t* na_bin) {
@@ -2095,6 +2207,16 @@ static int init_handle(ygg_gbt* h) {
   }
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_nodes_all, static_cast<size_t>(h->tree_capacity) * h->max_nodes));
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_nodes_scratch, h->max_nodes));
+  h->set_words = ds->set_words();
+  if (h->set_words > 0) {
+    // the positive sets of the wide categorical splits: (tree capacity + 1) x max_nodes / 2 x set_words x 4 B
+    const size_t words = (static_cast<size_t>(h->tree_capacity) + 1) * pool_nodes(h) * h->set_words;
+    if (dev_alloc(&h->d_sets, words) != YGG_OK) {
+      (void)cudaGetLastError();
+      return set_error(YGG_ERR_CUDA, "wide categorical columns: %.2f GB of positive-set pool ((%d trees + 1) x %d nodes x %d words) "
+                       "could not be allocated", static_cast<double>(words) * 4 / 1e9, h->tree_capacity, pool_nodes(h), h->set_words);
+    }
+  }
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_loss, h->tree_capacity));
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_loss_partials, 1));
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_ties, h->max_level_nodes));
@@ -2125,6 +2247,8 @@ int ygg_gbt_destroy(ygg_gbt* h) {
   dev_free(h->d_wsum); dev_free(h->d_wcnt); dev_free(h->d_whsum);
   for (int i = 0; i < 2; i++) { dev_free(h->d_wnode_sum[i]); dev_free(h->d_wnode_cnt[i]); dev_free(h->d_wnode_hsum[i]); }
   dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins);
+  dev_free(h->d_wide_cat); dev_free(h->d_wide_na_bin); dev_free(h->d_wide_set); dev_free(h->d_sort_key); dev_free(h->d_sort_idx);
+  dev_free(h->d_sets); dev_free(h->d_sort_off);
   cudaFree(h->d_goss_temp);
   cudaFree(h->d_level_buf);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -2429,7 +2553,7 @@ int attach_validation(ygg_gbt* h, const ygg_dataset* valid, int64_t n) {
   if (!h->has_labels) return set_error(YGG_ERR_INVALID_ARGUMENT, "set the training labels first (the initial prediction comes from them)");
   if (valid->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset lives on another device");
   if (valid->F != h->ds->F || valid->num_bins != h->ds->num_bins || valid->feature_type != h->ds->feature_type ||
-      valid->wide_feature != h->ds->wide_feature || valid->wide_bins != h->ds->wide_bins)
+      valid->wide_feature != h->ds->wide_feature || valid->wide_bins != h->ds->wide_bins || valid->wide_cat != h->ds->wide_cat)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset does not have the features / binning of the training dataset");
   if (n != valid->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "label count %lld != validation rows %lld", static_cast<long long>(n), static_cast<long long>(valid->n));
   YGG_CUDA(cudaSetDevice(h->ds->device));
@@ -2483,6 +2607,7 @@ int ygg_dataset_split_rows(const ygg_dataset* ds, const uint8_t* select, ygg_dat
     if (ds->n_wide() > 0) {   // the wide columns travel with the rows: codes, bucket values and NA replacements
       ygg_dataset* o = out[k];
       o->wide_of = ds->wide_of; o->wide_feature = ds->wide_feature; o->wide_bins = ds->wide_bins; o->wide_na_bin = ds->wide_na_bin;
+      o->wide_cat = ds->wide_cat;
       o->wide_off = ds->wide_off; o->wide_values = ds->wide_values; o->wide_na_replacement = ds->wide_na_replacement;
       st = dev_alloc(&o->d_wide, static_cast<size_t>(ds->n_wide()) * o->n_pad);
       if (st == YGG_OK) st = upload_wide_meta(o);
@@ -2777,6 +2902,42 @@ int ygg_gbt_get_tree(ygg_gbt* h, int32_t iter, ygg_node* out, int32_t capacity, 
   return YGG_OK;
 }
 
+int ygg_gbt_get_category_set(ygg_gbt* h, int32_t iter, int32_t node, uint32_t* words, int32_t capacity, int32_t* n_words) {
+  if (!h || !n_words) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (iter == -1 && !h->scratch_tree) return set_error(YGG_ERR_INVALID_ARGUMENT, "no tree grown by ygg_tree_train_on_gradients yet");
+  if (iter < -1 || iter >= h->trees_done) return set_error(YGG_ERR_INVALID_ARGUMENT, "tree %d not trained (have %d)", iter, h->trees_done);
+  YGG_CUDA(cudaSetDevice(h->ds->device));
+  if (iter >= 0) YGG_RETURN_IF_ERROR(resolve_ties(h, h->trees_done));
+  const NodeRec* d_tree = iter >= 0 ? h->d_nodes_all + static_cast<size_t>(iter) * h->max_nodes : h->d_nodes_scratch;
+  std::vector<NodeRec> nodes(h->max_nodes);
+  YGG_CUDA(cudaMemcpyAsync(nodes.data(), d_tree, sizeof(NodeRec) * h->max_nodes, cudaMemcpyDeviceToHost, h->stream));
+  YGG_CUDA(cudaStreamSynchronize(h->stream));
+  // the node id of pre-order index `node` (the order of ygg_gbt_get_tree: node, negative subtree, positive subtree)
+  std::vector<int> stack(1, 0);
+  int id = -1;
+  for (int k = 0; !stack.empty(); k++) {
+    const int i = stack.back();
+    stack.pop_back();
+    if (k == node) { id = i; break; }
+    if (nodes[i].feature >= 0) { stack.push_back(nodes[i].pos_child); stack.push_back(nodes[i].neg_child); }
+  }
+  if (id < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "tree %d has no node %d", iter, node);
+  const NodeRec& nd = nodes[id];
+  if (nd.feature < 0 || nd.cond_type != YGG_FEATURE_CATEGORICAL)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "node %d of tree %d is not a categorical split", node, iter);
+  const int wi = h->ds->wide_of.empty() ? -1 : h->ds->wide_of[nd.feature];
+  *n_words = wi >= 0 ? (h->ds->wide_bins[wi] + 31) / 32 : 8;
+  if (!words || capacity < *n_words) return set_error(YGG_ERR_INVALID_ARGUMENT, "capacity %d < %d words", capacity, *n_words);
+  if (wi < 0) {
+    std::memcpy(words, nd.mask, sizeof(nd.mask));
+    return YGG_OK;
+  }
+  YGG_CUDA(cudaMemcpyAsync(words, sets_of(h, d_tree) + static_cast<size_t>(id) * h->set_words, sizeof(uint32_t) * *n_words,
+                           cudaMemcpyDeviceToHost, h->stream));
+  YGG_CUDA(cudaStreamSynchronize(h->stream));
+  return YGG_OK;
+}
+
 int ygg_gbt_train_loss(ygg_gbt* h, int32_t iter, float* loss, float* secondary) {
   if (!h || !loss || !secondary) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (iter < 0 || iter >= h->iters_done) return set_error(YGG_ERR_INVALID_ARGUMENT, "iteration %d not trained", iter);
@@ -2806,7 +2967,7 @@ int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   if (!h || !ds || !out) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (ds->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset lives on another device");
   if (ds->F != h->ds->F || ds->num_bins != h->ds->num_bins || ds->feature_type != h->ds->feature_type ||
-      ds->wide_feature != h->ds->wide_feature || ds->wide_bins != h->ds->wide_bins)
+      ds->wide_feature != h->ds->wide_feature || ds->wide_bins != h->ds->wide_bins || ds->wide_cat != h->ds->wide_cat)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset does not have the features / binning of the training dataset");
   if (n != ds->n * h->K) return set_error(YGG_ERR_INVALID_ARGUMENT, "n mismatch (rows x classes expected)");
   YGG_CUDA(cudaSetDevice(h->ds->device));
@@ -2816,7 +2977,7 @@ int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   YGG_RETURN_IF_ERROR(dev_alloc(&d_out, static_cast<size_t>(n)));
   const int n_trees = ygg_gbt_num_trees(h);
   k_predict<<<static_cast<int>(std::min<int64_t>((ds->n + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 16)), 256, 0, h->stream>>>(
-      ds->d_bins, ds->d_wide, ds->d_wide_of, ds->n, ds->n_pad, h->d_nodes_all, h->max_nodes, n_trees, h->K, h->initial_prediction, d_out);
+      ds->d_bins, ds->d_wide, ds->d_wide_of, ds->n, ds->n_pad, h->d_nodes_all, h->d_sets, h->set_words, pool_nodes(h), h->max_nodes, n_trees, h->K, h->initial_prediction, d_out);
   h->launches_total++;
   int st = check_launch("k_predict");
   if (st == YGG_OK && (cudaMemcpyAsync(out, d_out, sizeof(float) * n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
@@ -2853,9 +3014,11 @@ int ygg_tree_train_on_gradients(ygg_gbt* h, const float* gradients, const float*
   k_absmax<<<elementwise_grid(h), 256, 0, h->stream>>>(h->d_g, n, h->d_st);
   h->launches_total++;
   YGG_RETURN_IF_ERROR(check_launch("k_absmax"));
+  h->scratch_tree = false;
   YGG_RETURN_IF_ERROR(grow_tree(h, h->d_nodes_scratch));
   if (h->cfg.growing_strategy == 1) YGG_RETURN_IF_ERROR(best_first_prune(h, h->d_nodes_scratch));
   YGG_RETURN_IF_ERROR(check_device_error(h));
+  h->scratch_tree = true;
   std::vector<ygg_node> flat;
   YGG_RETURN_IF_ERROR(fetch_tree(h, h->d_nodes_scratch, &flat, true));
   *n_nodes = static_cast<int32_t>(flat.size());
@@ -3174,9 +3337,31 @@ int ygg_gbt_save_ydf(ygg_gbt* h, const char* directory, const char* label_name, 
   std::vector<int64_t> offsets(1, 0);
   const int n_trees = ygg_gbt_num_trees(h), n_logs = ygg_gbt_num_iterations(h);
   std::vector<float> loss(n_logs), sec(n_logs), vloss, vsec;
+  const ygg_dataset* ds = h->ds;
+  std::vector<int32_t> num_values = ds->num_bins;   // a wide column's own bucket count
+  for (int w = 0; w < ds->n_wide(); w++) num_values[ds->wide_feature[w]] = ds->wide_bins[w];
+  std::vector<int64_t> set_offset;                  // wide categorical splits: their pooled sets
+  std::vector<uint32_t> set_words;
   for (int t = 0; t < n_trees; t++) {
+    const NodeRec* d_tree = h->d_nodes_all + static_cast<size_t>(t) * h->max_nodes;
     std::vector<ygg_node> flat;
-    YGG_RETURN_IF_ERROR(fetch_tree(h, h->d_nodes_all + static_cast<size_t>(t) * h->max_nodes, &flat));
+    YGG_RETURN_IF_ERROR(fetch_tree(h, d_tree, &flat));
+    if (h->d_sets != nullptr) {
+      std::vector<NodeRec> nodes(h->max_nodes);
+      std::vector<int> ids;
+      std::vector<uint32_t> pool(static_cast<size_t>(pool_nodes(h)) * h->set_words);
+      YGG_CUDA(cudaMemcpyAsync(nodes.data(), d_tree, sizeof(NodeRec) * h->max_nodes, cudaMemcpyDeviceToHost, h->stream));
+      YGG_CUDA(cudaMemcpyAsync(pool.data(), sets_of(h, d_tree), sizeof(uint32_t) * pool.size(), cudaMemcpyDeviceToHost, h->stream));
+      YGG_CUDA(cudaStreamSynchronize(h->stream));
+      preorder_ids(nodes, 0, &ids);
+      for (size_t i = 0; i < flat.size(); i++) {
+        const int wi = flat[i].feature >= 0 ? ds->wide_of[flat[i].feature] : -1;
+        if (wi < 0 || flat[i].condition_type != YGG_FEATURE_CATEGORICAL) { set_offset.push_back(-1); continue; }
+        set_offset.push_back(static_cast<int64_t>(set_words.size()));
+        const uint32_t* src = pool.data() + static_cast<size_t>(ids[i]) * h->set_words;
+        set_words.insert(set_words.end(), src, src + (ds->wide_bins[wi] + 31) / 32);
+      }
+    }
     all.insert(all.end(), flat.begin(), flat.end());
     offsets.push_back(static_cast<int64_t>(all.size()));
   }
@@ -3212,7 +3397,9 @@ int ygg_gbt_save_ydf(ygg_gbt* h, const char* directory, const char* label_name, 
   d.data_spec_len = data_spec_len;
   d.train_loss = loss.data();
   d.train_secondary = sec.data();
-  d.feature_num_values = h->ds->num_bins.data();
+  d.feature_num_values = num_values.data();
+  d.node_set_offset = set_offset.empty() ? nullptr : set_offset.data();
+  d.cat_set_words = set_words.data();
   const int st = ygg_model_write_ydf(&d);
   if (st != YGG_OK) return set_error(st, "could not write the model directory %s", directory);
   return YGG_OK;

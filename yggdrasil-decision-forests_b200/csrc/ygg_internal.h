@@ -1,5 +1,6 @@
 // ygg_internal.h — declarations shared by the translation units of libygg_b200.so (not part of the ABI).
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <vector>
 
@@ -27,10 +28,19 @@ struct ygg_dataset {
   int32_t* d_wide_of = nullptr;        // [F] wide index of a feature, -1 for a byte column
   int64_t* d_wide_off = nullptr;       // [wide features] offset of the feature's buckets in d_wide_values / the wide planes
   float* d_wide_values = nullptr;      // [sum of the wide features' buckets] bucket values (ascending per feature)
-  std::vector<int32_t> wide_of, wide_feature, wide_bins, wide_na_bin;
+  // Wide categorical columns (ygg_dataset_set_wide_categorical_column, DESIGN.md §21) share these tables: wide_cat[w] = 1,
+  // and their bucket values are zeros that nothing reads.
+  std::vector<int32_t> wide_of, wide_feature, wide_bins, wide_na_bin, wide_cat;
   std::vector<int64_t> wide_off;       // host copy of d_wide_off, plus the total at the end
   std::vector<float> wide_values, wide_na_replacement;
   int n_wide() const { return static_cast<int>(wide_feature.size()); }
+  // 32-bit words of the widest categorical wide column's positive set (0 without one)
+  int set_words() const {
+    int m = 0;
+    for (int w = 0; w < n_wide(); w++)
+      if (wide_cat[w]) m = std::max(m, (wide_bins[w] + 31) / 32);
+    return m;
+  }
   int handles = 0;                     // live ygg_gbt handles on this dataset (wide columns are set before the first)
 };
 

@@ -534,6 +534,21 @@ __device__ void scan_node(const ScanParams& p, const NodeRec& node, int f_global
   __syncthreads();
 }
 
+// The sort key of one category bucket (count, unbiased quantised sum, second-plane sum): the label mean (variance gain,
+// splitter_accumulator.h:1492-1494) or the float hessian priority (:1797-1804, :1699-1701); 0 for an empty bucket.
+// Shared by the byte scan (scan_node_categorical) and the wide categorical scan (k_scan_wide_cat, ygg_wide.cuh).
+__device__ __forceinline__ double category_key(const ScanParams& p, long long cnt, long long sq, long long hq, double ginv,
+                                               double hinv) {
+  if (!p.use_hessian) {
+    // Mean() = sum / count, count = the weight sum when weighted (distribution.h; 0 for an empty bucket)
+    const double den = p.weighted ? static_cast<double>(hq) * p.w_inv : static_cast<double>(cnt);
+    return (cnt == 0 || den == 0.0) ? 0.0 : (static_cast<double>(sq) * ginv) / den;
+  }
+  const double H = static_cast<double>(hq) * hinv;
+  return H > 0 ? static_cast<double>(static_cast<float>(l1_threshold_d(static_cast<double>(sq) * ginv, p.l1) / (H + p.l2_categorical)))
+               : 0.0;
+}
+
 // Categorical feature: FindBestSplit<..., require_label_sorting=true> (splitter_scanner.h:1823-1826,
 // :1978-1981).  The buckets (one per category) are sorted by label mean (variance gain,
 // splitter_accumulator.h:1492-1494) or by the float hessian priority (:1797-1804, :1699-1701), then
@@ -555,17 +570,8 @@ __device__ void scan_node_categorical(const ScanParams& p, const NodeRec& node, 
   const double ginv = static_cast<double>(p.st->g_pow2) / static_cast<double>(1u << (kQBits - 1));
   const double hinv = static_cast<double>(p.st->h_pow2) / static_cast<double>(1u << kQBits);
   const double l2 = p.l2_categorical;
-  double key;
-  if (b >= B) {
-    key = __longlong_as_double(0x7FF0000000000000ll);  // +inf: not a category of this feature
-  } else if (!p.use_hessian) {
-    // Mean() = sum / count, count = the weight sum when weighted (distribution.h; 0 for an empty bucket)
-    const double den = p.weighted ? static_cast<double>(hq) * p.w_inv : static_cast<double>(cnt);
-    key = (cnt == 0 || den == 0.0) ? 0.0 : (static_cast<double>(sq) * ginv) / den;
-  } else {
-    const double H = static_cast<double>(hq) * hinv;
-    key = H > 0 ? static_cast<double>(static_cast<float>(l1_threshold_d(static_cast<double>(sq) * ginv, p.l1) / (H + l2))) : 0.0;
-  }
+  const double key = b >= B ? __longlong_as_double(0x7FF0000000000000ll)   // +inf: not a category of this feature
+                            : category_key(p, cnt, sq, hq, ginv, hinv);
   s_key[b] = key; s_idx[b] = b; s_cnt[b] = cnt; s_sq[b] = sq; s_hq[b] = hq;
   if (b < 8) s_mask[b] = 0u;
   __syncthreads();
@@ -749,7 +755,19 @@ struct SelectParams {
   // wide columns (single GPU): the float thresholds k_scan_wide left per (level node, feature); null without wide columns
   const int32_t* wide_of;      // [F] wide index, -1 for a byte column
   const float* wide_thr_value; // [level nodes][f_count]
+  // wide categorical columns: the positive sets k_scan_wide_cat left per (level node, wide feature) (null without them)
+  const uint32_t* wide_set;    // [level nodes][n_wide][set_words]
+  const int32_t* wide_na_bin;  // [n_wide]
+  int n_wide, set_words;
 };
+
+// Candidate (level node j, wide index wi) is a wide categorical one: its positive set is in p.wide_set.
+__device__ __forceinline__ const uint32_t* wide_set_of(const SelectParams& p, int j, int wi) {
+  return p.wide_set + (static_cast<size_t>(j) * p.n_wide + wi) * p.set_words;
+}
+__device__ __forceinline__ int wide_cat_index(const SelectParams& p, int fg, int cond_type) {
+  return (p.wide_set != nullptr && cond_type == 1) ? p.wide_of[fg] : -1;
+}
 
 // The float threshold of candidate (level node j, local feature fl): a wide column's from k_scan_wide's side array, a
 // lossless byte column's from its packed threshold, NaN for a discretized one.
@@ -810,6 +828,9 @@ __global__ void __launch_bounds__(256) k_select_local(SelectParams p) {
               const int na = p.na_bin[fg];
               for (int i = 0; i < 8; i++) a.mask[i] = m[i];
               a.na_value = (m[na >> 5] >> (na & 31)) & 1u;
+              // a wide categorical alternative does not carry its set: it is never verified, so the tie-break replay
+              // keeps the engine's choice and counts the node as unresolved when the reference would take it
+              if (wide_cat_index(p, fg, 1) >= 0) a.n_pos = -1;
             } else {
               a.na_value = (p.na_bin[fg] >= a.thr) ? 1 : 0;   // na_bin > thr - 1
               if (a.thr_value == a.thr_value) a.na_value = p.na_replacement[fg] >= a.thr_value ? 1 : 0;   // exact rule (:218)
@@ -834,6 +855,11 @@ __global__ void __launch_bounds__(256) k_select_local(SelectParams p) {
 #pragma unroll
           for (int i = 0; i < 8; i++) out.mask[i] = m[i];
           out.na_value = (m[na >> 5] >> (na & 31)) & 1u;  // NA replacement in the positive set
+          const int wi = wide_cat_index(p, fg, 1);
+          if (wi >= 0) {   // (its byte mask is the filler's: empty)
+            const int wna = p.wide_na_bin[wi];
+            out.na_value = (wide_set_of(p, j, wi)[wna >> 5] >> (wna & 31)) & 1u;
+          }
         }
       }
       p.shard_best[static_cast<size_t>(p.rank) * p.max_level_nodes + j] = out;
@@ -1051,6 +1077,8 @@ struct PartParams {
   int smem_children_private;  // capacity with one accumulator copy per lane
   const uint16_t* wide;       // k_partition_wide: the dataset's wide columns (ygg_dataset.d_wide / d_wide_of)
   const int32_t* wide_of;
+  const uint32_t* sets;       // k_partition_wide: the tree's positive-set pool [max_nodes][set_words] (wide categorical splits)
+  int set_words;
 };
 
 // Shared accumulators per child: cnt, g_lo, g_hi, h_lo, h_hi, g2_lo, g2_hi.
@@ -1201,6 +1229,9 @@ __device__ __forceinline__ void partition_impl(const PartParams& p) {
             bool go_pos;
             if (!CAT || pn.thr >= 0) {
               go_pos = static_cast<int>(bin) >= pn.thr;
+            } else if (WIDE && p.wide_of[pn.feature] >= 0) {   // a wide categorical split: its set in the pool
+              const uint32_t mw = p.sets[static_cast<size_t>(lv.first_node + li) * p.set_words + (bin >> 5)];
+              go_pos = ((mw >> (bin & 31)) & 1u) != 0;
             } else {
               const uint32_t mw = nodes_in_smem ? s_masks[li][bin >> 5] : p.nodes[lv.first_node + li].mask[bin >> 5];
               go_pos = ((mw >> (bin & 31)) & 1u) != 0;
@@ -1531,7 +1562,8 @@ __global__ void __launch_bounds__(1024) k_weight_sums_finish(WeightSumParams p) 
 // the node to the same side (twin columns); equal float scores and equal positive counts do not prove that.  Every
 // row walks from its leaf to the root; at each ancestor with recorded ties it knows on which side it went and
 // evaluates the alternatives' conditions: a disagreement disqualifies the alternative (n_pos = -1).
-// (`wide` / `wide_of`: the dataset's wide columns, null without them)
+// (`wide` / `wide_of`: the dataset's wide columns, null without them.  A wide categorical alternative is recorded with
+// n_pos = -1 by k_select_local: it is never evaluated here.)
 __global__ void __launch_bounds__(256) k_verify_ties(NodeRec* nodes, const uint16_t* __restrict__ node_of_row,
                                                      const uint8_t* __restrict__ bins, int64_t n, int64_t n_pad,
                                                      const uint16_t* __restrict__ wide, const int32_t* __restrict__ wide_of) {

@@ -43,8 +43,9 @@ bool write_file(const std::string& path, const std::string& data) {
 }
 
 // decision_tree::proto::Node for one flat node (model/decision_tree/decision_tree.proto).
+// `set`: the positive set of a wide categorical split (null: n.cat_mask, 256 categories at most).
 std::string encode_node(const ygg_node& n, int use_hessian_gain, const int32_t* feature_col_idx,
-                        const int32_t* feature_num_values) {
+                        const int32_t* feature_num_values, const uint32_t* set) {
   Pb reg;  // NodeRegressorOutput
   reg.f32(1, n.leaf_value);  // top_value
   if (use_hessian_gain) {
@@ -66,20 +67,23 @@ std::string encode_node(const ygg_node& n, int use_hessian_gain, const int32_t* 
       // SetPositiveAttributeSetOfCategoricalContainsCondition (learner/decision_tree/utils.cc:31-63):
       // the smaller of a bitmap over the categories and a sorted int32 vector.
       const int num_values = feature_num_values ? feature_num_values[n.feature] : 256;
+      const uint32_t* words = set != nullptr ? set : n.cat_mask;
+      const int limit = set != nullptr ? num_values : 256;   // categories the set holds
+      auto positive = [&](int c) { return ((words[c >> 5] >> (c & 31)) & 1u) != 0; };
       int num_positive = 0;
-      for (int c = 0; c < 256; c++) num_positive += (n.cat_mask[c >> 5] >> (c & 31)) & 1u;
+      for (int c = 0; c < limit; c++) num_positive += positive(c) ? 1 : 0;
       const int64_t usage_bitmap = (num_values + 7) / 8, usage_vector = 4 * static_cast<int64_t>(num_positive);
       if (usage_bitmap <= usage_vector) {
         std::string bitmap(static_cast<size_t>(usage_bitmap), '\0');
-        for (int c = 0; c < num_values && c < 256; c++)
-          if ((n.cat_mask[c >> 5] >> (c & 31)) & 1u) bitmap[c / 8] = static_cast<char>(bitmap[c / 8] | (1 << (c & 7)));
+        for (int c = 0; c < num_values && c < limit; c++)
+          if (positive(c)) bitmap[c / 8] = static_cast<char>(bitmap[c / 8] | (1 << (c & 7)));
         Pb cb;  // Condition.ContainsBitmap
         cb.bytes(1, bitmap);  // elements_bitmap
         cond.msg(5, cb);      // contains_bitmap_condition
       } else {
         Pb packed;
-        for (int c = 0; c < 256; c++)
-          if ((n.cat_mask[c >> 5] >> (c & 31)) & 1u) packed.varint(static_cast<uint64_t>(c));
+        for (int c = 0; c < limit; c++)
+          if (positive(c)) packed.varint(static_cast<uint64_t>(c));
         Pb cv;  // Condition.ContainsVector
         cv.bytes(1, packed.s);  // elements, packed
         cond.msg(4, cv);        // contains_condition
@@ -172,7 +176,9 @@ extern "C" int ygg_model_write_ydf(const ygg_model_desc* d) {
   blob.append(reinterpret_cast<const char*>(file_header), 8);
   for (int t = 0; t < d->num_trees; t++) {
     for (int64_t i = d->tree_offsets[t]; i < d->tree_offsets[t + 1]; i++) {
-      const std::string rec = encode_node(d->trees[i], d->use_hessian_gain, d->feature_col_idx, d->feature_num_values);
+      const int64_t so = d->node_set_offset != nullptr ? d->node_set_offset[i] : -1;
+      const uint32_t* set = (so >= 0 && d->cat_set_words != nullptr) ? d->cat_set_words + so : nullptr;
+      const std::string rec = encode_node(d->trees[i], d->use_hessian_gain, d->feature_col_idx, d->feature_num_values, set);
       const uint32_t len = static_cast<uint32_t>(rec.size());
       blob.append(reinterpret_cast<const char*>(&len), 4);  // little endian on every supported host
       blob.append(rec);

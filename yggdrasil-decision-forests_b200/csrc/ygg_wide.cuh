@@ -66,6 +66,14 @@ struct WideScanParams {
   const uint32_t* pnode_cnt;
   const unsigned long long* pnode_hsum;
   float* thr_value;              // [level nodes][f_count] float threshold of the wide candidates (SelectParams.wide_thr_value)
+  // wide categorical columns (k_scan_wide_cat; null / 0 without them)
+  const int32_t* wide_cat;       // [wide features] 1: categorical
+  int n_wide, set_words;
+  uint32_t* set_out;             // [level nodes][n_wide][set_words] positive sets (SelectParams.wide_set)
+  double* sort_key;              // [grid.x][sort_total] per-CTA sort scratch: feature w's block of sort_pad(B_w) entries
+  int32_t* sort_idx;             // starts at sort_off[w]
+  const int64_t* sort_off;       // [wide features]
+  int64_t sort_total;
 };
 
 // Bucket b of a node: the direct histogram (slot plane at `d`), or parent (node plane at `x`) - direct.  Sums unbiased.
@@ -187,6 +195,7 @@ __global__ void __launch_bounds__(256) k_scan_wide(WideScanParams p) {
   if (static_cast<int>(blockIdx.x) >= lv.num_families) return;
   const Family fam = p.s.families[blockIdx.x];
   const int w = blockIdx.y;
+  if (p.wide_cat != nullptr && p.wide_cat[w]) return;   // k_scan_wide_cat's
   const int f = p.wide_feature[w];
   const int fl = f - p.s.f_begin;
   const int B = p.wide_bins[w];
@@ -206,6 +215,175 @@ __global__ void __launch_bounds__(256) k_scan_wide(WideScanParams p) {
       scan_wide_node<HESS>(p, fam.derived, fl, B, values, d, x, true, xn, p.s.write_derived != 0);
     }
   }
+}
+
+// Wide categorical columns (DESIGN.md §21): scan_node_categorical for B = 257..65535 buckets.  The keys (category_key),
+// sorted ascending by (key, category index) with a bitonic sort over the CTA's global scratch (`key` / `idx`,
+// sort_pad(B) entries, +inf past B), then the sorted buckets scanned in tiles of 256 with a running carry and scored by
+// boundary_score with l2_categorical; the first maximum wins.  The categories after the best boundary form the positive
+// set, written to p.set_out.
+// Entries of the sort scratch of a categorical column of B categories: the power of two >= B.
+__host__ __device__ inline int sort_pad(int B) {
+  int P = 1;
+  while (P < B) P <<= 1;
+  return P;
+}
+
+template <bool HESS>
+__device__ void scan_wide_cat_node(const WideScanParams& p, int node, int fl, int w, int B, size_t d, size_t x, bool derived,
+                                   size_t copy_to, bool copy, double* key, int32_t* idx) {
+  __shared__ Scan3 s_warp[8];
+  __shared__ double s_best_score[8];
+  __shared__ int s_best_b[8];
+  __shared__ long long s_npos;
+  const LevelDesc lv = p.s.levels[p.s.level];
+  const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5;
+  const int P = sort_pad(B);
+  const double ginv = static_cast<double>(p.s.st->g_pow2) / static_cast<double>(1u << (kQBits - 1));
+  const double hinv = static_cast<double>(p.s.st->h_pow2) / static_cast<double>(1u << kQBits);
+  // pass 1: the node's totals (and its copy for the next level), the keys
+  Scan3 mine{0, 0, 0};
+  for (int b = tid; b < P; b += blockDim.x) {
+    double k = __longlong_as_double(0x7FF0000000000000ll);   // +inf: past the feature's categories
+    if (b < B) {
+      const Scan3 v = wide_bucket<HESS>(p, d, x, derived, b);
+      mine.c += v.c; mine.s += v.s; mine.h += v.h;
+      if (copy) {
+        p.node_cnt[copy_to + b] = static_cast<uint32_t>(v.c);
+        p.node_sum[copy_to + b] = static_cast<unsigned long long>(v.s + v.c * static_cast<long long>(kQBias));
+        if (HESS && p.s.has_h) p.node_hsum[copy_to + b] = static_cast<unsigned long long>(v.h);
+      }
+      k = category_key(p.s, v.c, v.s, v.h, ginv, hinv);
+    }
+    key[b] = k;
+    idx[b] = b;
+  }
+  Scan3 tot;
+  block_inclusive_scan(mine, s_warp, &tot);
+  __syncthreads();
+  // bitonic sort of (key, index) pairs, ascending; -0.0 == +0.0, equal keys in index order
+  for (int k = 2; k <= P; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < P; i += blockDim.x) {
+        const int partner = i ^ j;
+        if (partner > i) {
+          const double ka = key[i], kb = key[partner];
+          const int ia = idx[i], ib = idx[partner];
+          const bool a_gt_b = ka > kb || (ka == kb && ia > ib);
+          if (a_gt_b == ((i & k) == 0)) { key[i] = kb; key[partner] = ka; idx[i] = ib; idx[partner] = ia; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  // pass 2: every boundary between sorted positions, tile by tile with a running carry
+  ScanParams sp = p.s;
+  sp.l2 = p.s.l2_categorical;
+  double bs = -1.0;
+  int bb = 0x7fffffff;
+  long long bnpos = 0;
+  Scan3 carry{0, 0, 0};
+  for (int t0 = 0; t0 < B; t0 += blockDim.x) {
+    const int pos = t0 + tid;
+    const Scan3 v = pos < B ? wide_bucket<HESS>(p, d, x, derived, idx[pos]) : Scan3{0, 0, 0};
+    Scan3 tile;
+    Scan3 inc = block_inclusive_scan(v, s_warp, &tile);
+    inc.c += carry.c; inc.s += carry.s; inc.h += carry.h;
+    carry.c += tile.c; carry.s += tile.s; carry.h += tile.h;
+    double score;
+    if (boundary_score(sp, tot, inc, pos <= B - 2, ginv, hinv, &score) && score > bs) { bs = score; bb = pos; bnpos = tot.c - inc.c; }
+  }
+  const int my_b = bb;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double os = __shfl_xor_sync(0xffffffffu, bs, o);
+    const int ob = __shfl_xor_sync(0xffffffffu, bb, o);
+    if (os > bs || (os == bs && ob < bb)) { bs = os; bb = ob; }
+  }
+  if (lane == 0) { s_best_score[wp] = bs; s_best_b[wp] = bb; }
+  __syncthreads();
+  bs = s_best_score[0]; bb = s_best_b[0];
+  for (int i = 1; i < 8; i++)
+    if (s_best_score[i] > bs || (s_best_score[i] == bs && s_best_b[i] < bb)) { bs = s_best_score[i]; bb = s_best_b[i]; }
+  const bool found = bb != 0x7fffffff;
+  if (found && my_b == bb) s_npos = bnpos;
+  // pass 3: the positive set = the categories at sorted positions after the best boundary
+  const size_t j = static_cast<size_t>(node - lv.first_node);
+  uint32_t* set = p.set_out + (j * p.n_wide + w) * p.set_words;
+  for (int i = tid; i < p.set_words; i += blockDim.x) set[i] = 0u;
+  __syncthreads();
+  if (found)
+    for (int pos = bb + 1 + tid; pos < B; pos += blockDim.x) {
+      const int c = idx[pos];
+      atomicOr(&set[c >> 5], 1u << (c & 31));
+    }
+  if (tid == 0) {
+    const size_t ci = j * p.s.f_count + fl;
+    Candidate c{0.f, 0, 0, 0};
+    if (found) {
+      c.found = 1;
+      c.score = static_cast<float>(bs);
+      c.n_pos = static_cast<int32_t>(s_npos);
+    }
+    p.s.cand[ci] = c;
+    p.thr_value[ci] = __builtin_nanf("");
+  }
+  __syncthreads();   // the scratch is reused by the CTA's next node
+}
+
+// One CTA of 256 threads per (family, wide categorical feature), launched next to k_scan_wide (which skips these
+// features); same planes, same ping-pong copies.
+template <bool HESS>
+__global__ void __launch_bounds__(256) k_scan_wide_cat(WideScanParams p) {
+  const LevelDesc lv = p.s.levels[p.s.level];
+  if (static_cast<int>(blockIdx.x) >= lv.num_families) return;
+  const int w = blockIdx.y;
+  if (!p.wide_cat[w]) return;
+  const Family fam = p.s.families[blockIdx.x];
+  const int fl = p.wide_feature[w] - p.s.f_begin;
+  const int B = p.wide_bins[w];
+  const int64_t off = p.off[w];
+  double* key = p.sort_key + static_cast<size_t>(blockIdx.x) * p.sort_total + p.sort_off[w];
+  int32_t* idx = p.sort_idx + static_cast<size_t>(blockIdx.x) * p.sort_total + p.sort_off[w];
+  const NodeRec direct = p.s.nodes[fam.direct];
+  const size_t d = static_cast<size_t>(direct.slot) * p.total + off;
+  const size_t dn = static_cast<size_t>(fam.direct - lv.first_node) * p.total + off;
+  if (direct.candidate) scan_wide_cat_node<HESS>(p, fam.direct, fl, w, B, d, 0, false, dn, p.s.write_derived != 0, key, idx);
+  if (fam.derived >= 0) {
+    const NodeRec derived = p.s.nodes[fam.derived];
+    if (derived.candidate) {
+      const LevelDesc plv = p.s.levels[p.s.level - 1];
+      const size_t x = static_cast<size_t>(fam.parent - plv.first_node) * p.total + off;
+      const size_t xn = static_cast<size_t>(fam.derived - lv.first_node) * p.total + off;
+      scan_wide_cat_node<HESS>(p, fam.derived, fl, w, B, d, x, true, xn, p.s.write_derived != 0, key, idx);
+    }
+  }
+}
+
+// After k_select_global: a node of the level split on a wide categorical feature gets its positive set copied from the
+// level's side array into the tree's pool [max_nodes][set_words] (one CTA per level node).
+__global__ void __launch_bounds__(256) k_store_sets(const NodeRec* __restrict__ nodes, const LevelDesc* __restrict__ levels,
+                                                    int level, const int32_t* __restrict__ wide_of,
+                                                    const uint32_t* __restrict__ wide_set, int n_wide, int set_words,
+                                                    uint32_t* __restrict__ pool) {
+  const LevelDesc lv = levels[level];
+  const int j = blockIdx.x;
+  if (j >= lv.num_nodes) return;
+  const NodeRec& nd = nodes[lv.first_node + j];
+  if (nd.feature < 0 || nd.cond_type != 1) return;
+  const int wi = wide_of[nd.feature];
+  if (wi < 0) return;
+  const uint32_t* src = wide_set + (static_cast<size_t>(j) * n_wide + wi) * set_words;
+  uint32_t* dst = pool + static_cast<size_t>(lv.first_node + j) * set_words;
+  for (int i = threadIdx.x; i < set_words; i += blockDim.x) dst[i] = src[i];
+}
+
+// Whether row code `b` of split node `nd` goes to the positive child: the pooled set of a wide categorical split
+// (`set`: the node's pool entry; wide = the split feature is a wide column), else the byte mask or the threshold.
+__device__ __forceinline__ bool split_goes_pos(const NodeRec& nd, uint32_t b, bool wide, const uint32_t* set) {
+  if (nd.cond_type != 1) return static_cast<int>(b) >= nd.thr;
+  const uint32_t word = wide ? set[b >> 5] : nd.mask[b >> 5];
+  return ((word >> (b & 31)) & 1u) != 0;
 }
 
 }  // namespace ygg

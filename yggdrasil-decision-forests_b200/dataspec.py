@@ -64,12 +64,26 @@ class CategoricalColumn:
     num_values: int = 0
     feature_type = _capi.FEATURE_CATEGORICAL
 
-    def encode(self, values) -> np.ndarray:
+    @property
+    def wide(self) -> bool:
+        """More categories than a byte holds: a wide categorical column (_capi.Dataset.set_wide_categorical_column)."""
+        return self.num_bins > 256
+
+    def _codes(self, values, dtype) -> np.ndarray:
         index = {k: i for i, k in enumerate(self.vocabulary) if i > 0}
         keys, na = _categorical_keys(values)
-        out = np.fromiter((index.get(k, 0) for k in keys), dtype=np.uint8, count=len(keys))
+        out = np.fromiter((index.get(k, 0) for k in keys), dtype=dtype, count=len(keys))
         out[na] = self.na_bin
         return out
+
+    def encode(self, values) -> np.ndarray:
+        return self._codes(values, np.uint8)
+
+    def encode16(self, values) -> np.ndarray:
+        """uint16 codes by encode's rule (dictionary index, 0 = out-of-dictionary, missing -> na_bin), up to 65535."""
+        if self.num_bins > 65535:
+            raise ValueError(f"column {self.name!r}: {self.num_bins} categories do not fit uint16 codes below 65535")
+        return self._codes(values, np.uint16)
 
 
 def _categorical_keys(values):
@@ -119,10 +133,10 @@ def infer_categorical_column(name: str, values, min_vocab_frequency: int = 5, ma
         items = items[:limit]
     vocabulary = ["<OOD>"] + [k.decode() for _, k in items]
     counts = [ood] + [c for c, _ in items]
-    if len(vocabulary) > 256:
+    if len(vocabulary) > 65535:
         raise NotImplementedError(
-            f"column {name!r}: {len(vocabulary)} categories do not fit the engine's uint8 bins "
-            "(raise min_vocab_frequency or lower max_vocab_count)")
+            f"column {name!r}: {len(vocabulary)} categories do not fit the engine's uint16 codes (at most 65535; "
+            "raise min_vocab_frequency or lower max_vocab_count)")
     if pydf:
         most_frequent = 0
     else:
@@ -225,7 +239,7 @@ def encode_features(cols: Dict[str, np.ndarray], columns: Sequence[DiscretizedCo
 
 def device_dataset(bins: np.ndarray, columns: Sequence, device: int = 0) -> "_capi.Dataset":
     """The device dataset of encode_features' output: byte columns as they are, wide columns (more than 256 buckets)
-    attached with their codes, bucket values and mean."""
+    attached with their codes (and, numerical, their bucket values and mean)."""
     wide = [i for i, c in enumerate(columns) if c.num_bins > 256]
     byte_bins = np.zeros(bins.shape, np.uint8) if bins.dtype != np.uint8 else bins
     if bins.dtype != np.uint8:
@@ -237,7 +251,10 @@ def device_dataset(bins: np.ndarray, columns: Sequence, device: int = 0) -> "_ca
     try:
         for i in wide:
             c = columns[i]
-            ds.set_wide_column(i, bins[i], c.num_bins, c.na_bin, c.bucket_values, c.mean)
+            if c.feature_type == _capi.FEATURE_CATEGORICAL:
+                ds.set_wide_categorical_column(i, bins[i], c.num_bins, c.na_bin)
+            else:
+                ds.set_wide_column(i, bins[i], c.num_bins, c.na_bin, c.bucket_values, c.mean)
     except Exception:
         ds.close()
         raise

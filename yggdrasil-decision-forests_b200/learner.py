@@ -42,6 +42,7 @@ class GradientBoostedTreesLearner:
                  min_vocab_frequency: int = 5,
                  max_vocab_count: int = 2000,
                  categorical_algorithm: str = "CART",
+                 categorical_arity_limit_for_random: int = 300,
                  num_trees: int = 300,
                  shrinkage: float = 0.1,
                  max_depth: int = 6,
@@ -80,6 +81,16 @@ class GradientBoostedTreesLearner:
         self.max_vocab_count = int(max_vocab_count)
         if categorical_algorithm != "CART":
             raise NotImplementedError("only categorical_algorithm=CART is implemented")
+        # The reference's Categorical.arity_limit_for_random (decision_tree.proto:573-576, default 300): a column with at
+        # least that many categories is split with the RANDOM algorithm whatever categorical_algorithm says
+        # (training.cc:3214-3217, :3292-3295).  RANDOM is not built (DESIGN.md §21), so such columns are refused, not
+        # approximated; raising the limit asks the reference for CART on them too, which is what the engine computes.
+        if isinstance(categorical_arity_limit_for_random, bool) or \
+                not isinstance(categorical_arity_limit_for_random, (int, np.integer)):
+            raise TypeError("categorical_arity_limit_for_random must be an integer")
+        if int(categorical_arity_limit_for_random) < 1:
+            raise ValueError("categorical_arity_limit_for_random must be >= 1")
+        self.categorical_arity_limit_for_random = int(categorical_arity_limit_for_random)
         # weights: name of a numerical column holding one non-negative weight per example (PYDF's `weights` argument ->
         # TrainingConfig.weight_definition); the column is not a feature.  Implemented for the variance gain, all three
         # losses (ygg_gbt_set_weights_f32).
@@ -180,7 +191,20 @@ class GradientBoostedTreesLearner:
         if self.weights is not None and self.weights in names:
             raise ValueError(f'the weight column "{self.weights}" cannot be a feature')
         n = len(cols[self.label])
-        lossless = {}
+        lossless, categorical = {}, {}
+        for name in names:   # string columns -> CATEGORICAL (PYDF's semantic inference), checked before the device
+            if cols[name].dtype.kind in "OUS":
+                # this learner mirrors PYDF, whose string columns keep most_frequent_value = 0 (dataspec.py)
+                c = ds_lib.infer_categorical_column(name, cols[name], self.min_vocab_frequency, self.max_vocab_count,
+                                                    self.max_rows_stats, ds_lib.FRONT_END_PYDF)
+                if c.num_bins >= self.categorical_arity_limit_for_random:
+                    raise NotImplementedError(
+                        f'column "{name}" has {c.num_bins} categories (with <OOD>), at least '
+                        f"categorical_arity_limit_for_random (= {self.categorical_arity_limit_for_random}): the reference "
+                        "splits such columns with its random-mask algorithm, which is not built.  Raise "
+                        "categorical_arity_limit_for_random to split them with CART (the reference's result for that "
+                        "setting), or lower max_vocab_count / raise min_vocab_frequency")
+                categorical[name] = c
         if not self.discretize_numerical_columns:   # checked before anything is created on the device
             for name in names:
                 if cols[name].dtype.kind in "fiub":
@@ -198,11 +222,12 @@ class GradientBoostedTreesLearner:
         try:
             for f, name in enumerate(names):
                 v = cols[name]
-                if v.dtype.kind in "OUS":  # strings -> CATEGORICAL (PYDF's semantic inference)
-                    # this learner mirrors PYDF, whose string columns keep most_frequent_value = 0 (dataspec.py)
-                    c = ds_lib.infer_categorical_column(name, v, self.min_vocab_frequency, self.max_vocab_count,
-                                                        self.max_rows_stats, ds_lib.FRONT_END_PYDF)
-                    builder.add_bins(f, c.encode(v), c.num_bins, c.na_bin, _capi.FEATURE_CATEGORICAL)
+                if v.dtype.kind in "OUS":
+                    c = categorical[name]
+                    if c.wide:   # attached after finish(); the byte column is a placeholder
+                        builder.add_bins(f, np.zeros(n, np.uint8), 1, 0, _capi.FEATURE_CATEGORICAL)
+                    else:
+                        builder.add_bins(f, c.encode(v), c.num_bins, c.na_bin, _capi.FEATURE_CATEGORICAL)
                     columns[f] = c
                 elif v.dtype.kind not in "fiub":
                     raise NotImplementedError(f'column "{name}" has unsupported dtype {v.dtype}')
@@ -230,6 +255,9 @@ class GradientBoostedTreesLearner:
                                                       num_bins=len(bounds) + 1, na_bin=na_bin,
                                                       num_missing=int(missing), num_values=n)
             dataset = builder.finish()
+            for f, c in enumerate(columns):
+                if c.feature_type == _capi.FEATURE_CATEGORICAL and c.wide:
+                    dataset.set_wide_categorical_column(f, c.encode16(cols[c.name]), c.num_bins, c.na_bin)
             for f, c in enumerate(columns):   # exact numerical splitter: thresholds between the values present in a node
                 if getattr(c, "bucket_values", None) is None:
                     continue
@@ -331,6 +359,7 @@ class GradientBoostedTreesLearner:
                     gbt.set_validation(valid_ds, valid_labels, weights=valid_weights)
                 gbt.train(self.cfg.num_trees)
                 trees = [gbt.get_tree(i) for i in range(gbt.num_trees())]
+                category_sets = [gbt.get_category_sets(i, t) for i, t in enumerate(trees)]
                 logs = []
                 for i in range(gbt.num_iterations()):
                     l, s = gbt.train_loss(i)
@@ -347,6 +376,7 @@ class GradientBoostedTreesLearner:
                 if d is not None:
                     d.close()
         model = GradientBoostedTreesModel(spec, trees, init, self.loss, logs,
-                                          config={k: getattr(self.cfg, k) for k, _ in self.cfg._fields_})
+                                          config={k: getattr(self.cfg, k) for k, _ in self.cfg._fields_},
+                                          category_sets=category_sets)
         model.validation_loss, model.early_stopping_triggered = final
         return model

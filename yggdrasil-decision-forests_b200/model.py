@@ -15,9 +15,12 @@ from . import dataspec as ds_lib
 
 class GradientBoostedTreesModel:
     def __init__(self, spec: ds_lib.DataSpec, trees: List[np.ndarray], initial_prediction: float,
-                 loss: str, training_logs=None, config=None):
+                 loss: str, training_logs=None, config=None, category_sets=None):
         self.data_spec = spec
         self.trees = trees
+        # per tree {pre-order node index: uint32 words}: the positive sets of the splits on wide categorical columns
+        # (more than 256 categories), whose cat_mask is empty
+        self.category_sets = category_sets or [{} for _ in trees]
         self.initial_prediction = float(initial_prediction)
         self.loss = loss
         self.training_logs = training_logs or []
@@ -48,6 +51,13 @@ class GradientBoostedTreesModel:
         acc = np.full((n, k), self.initial_prediction, dtype=np.float32)
         rows = np.arange(n)
         for ti, t in enumerate(self.trees):
+            # the positive set of every node, words [nodes, width]: cat_mask, or the node's set from category_sets
+            sets = self.category_sets[ti]
+            width = max([8] + [len(w) for w in sets.values()])
+            words = np.zeros((len(t), width), np.uint32)
+            words[:, :8] = t["cat_mask"]
+            for node_i, w in sets.items():
+                words[node_i, :len(w)] = w
             node = np.zeros(n, dtype=np.int64)
             active = t["feature"][node] >= 0
             while active.any():
@@ -55,9 +65,9 @@ class GradientBoostedTreesModel:
                 nd = node[idx]
                 f = t["feature"][nd]
                 b = bins[f, idx].astype(np.int64)
-                # (the mask is only read for categorical conditions, whose bins are bytes; a wide column's code may not be)
-                in_set = (t["cat_mask"][nd, np.minimum(b >> 5, 7)] >> (b & 31).astype(np.uint32)) & 1
-                go_pos = np.where(t["condition_type"][nd] == 1, in_set != 0, b >= t["threshold_bin"][nd])
+                cat = t["condition_type"][nd] == 1   # (a categorical code is below its column's num_bins <= 32 x width)
+                go_pos = b >= t["threshold_bin"][nd]
+                go_pos[cat] = ((words[nd[cat], b[cat] >> 5] >> (b[cat] & 31).astype(np.uint32)) & 1) != 0
                 node[idx] = np.where(go_pos, t["pos_child"][nd], t["neg_child"][nd])
                 active = t["feature"][node] >= 0
             acc[:, ti % k] += t["leaf_value"][node]

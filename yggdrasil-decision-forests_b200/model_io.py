@@ -145,6 +145,7 @@ class ModelDesc(C.Structure):
         ("valid_secondary", C.POINTER(C.c_float)), ("has_validation_loss", C.c_int32),
         ("validation_loss", C.c_float), ("early_stopping_triggered", C.c_int32),
         ("num_trees_per_iter", C.c_int32), ("feature_num_values", C.POINTER(C.c_int32)),
+        ("node_set_offset", C.POINTER(C.c_int64)), ("cat_set_words", C.POINTER(C.c_uint32)),
     ]
 
 
@@ -185,6 +186,19 @@ def save_ydf_model(model, path: str):
         d.early_stopping_triggered = int(bool(getattr(model, "early_stopping_triggered", False)))
     nvals = np.asarray([c.num_bins for c in model.data_spec.columns], dtype=np.int32)
     d.feature_num_values = nvals.ctypes.data_as(C.POINTER(C.c_int32))
+    # positive sets of the splits on wide categorical columns
+    sets = getattr(model, "category_sets", None) or [{} for _ in model.trees]
+    set_off = np.full(len(trees), -1, dtype=np.int64)
+    chunks, used = [], 0
+    for t, tree_sets in enumerate(sets):
+        for node, words in sorted(tree_sets.items()):
+            set_off[offs[t] + node] = used
+            chunks.append(np.asarray(words, dtype=np.uint32))
+            used += len(chunks[-1])
+    words_all = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros(1, np.uint32))
+    if chunks:
+        d.node_set_offset = set_off.ctypes.data_as(C.POINTER(C.c_int64))
+        d.cat_set_words = words_all.ctypes.data_as(C.POINTER(C.c_uint32))
     st = _capi.lib().ygg_model_write_ydf(C.byref(d))
     if st != 0:
         raise _capi.YggError(st, f"could not write the model to {path}")
