@@ -115,8 +115,10 @@ enum ygg_early_stopping {
  * Mirrors proto::Node + proto::NodeCondition (model/decision_tree/decision_tree.proto). */
 enum ygg_feature_type {
   YGG_FEATURE_DISCRETIZED_NUMERICAL = 0, /* condition: bin >= threshold_bin */
-  YGG_FEATURE_CATEGORICAL = 1            /* condition: category in cat_mask (CART); a wide categorical column's set
+  YGG_FEATURE_CATEGORICAL = 1,           /* condition: category in cat_mask (CART); a wide categorical column's set
                                             is read with ygg_gbt_get_category_set */
+  YGG_FEATURE_NUMERICAL = 2              /* presorted numerical column (ygg_dataset_set_numerical_column): condition
+                                            value >= threshold_value (threshold_bin = -1), a missing value -> na_value */
 };
 
 typedef struct ygg_node {
@@ -206,6 +208,19 @@ int ygg_dataset_set_wide_categorical_column(ygg_dataset* ds, int32_t feature, co
                                             int32_t na_bin);
 /* Read-back of a wide column: codes[n_rows], and (may be NULL) its num_bins / na_bin. */
 int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t* codes, int32_t* num_bins, int32_t* na_bin);
+/* Presorted numerical column (DESIGN.md §22): a numerical feature stored as its float values, with no limit on its
+ * distinct values.  It is split by the reference's exact numerical splitter (ScanSplitsPresortedSparse,
+ * splitter_scanner.h:1232-1430) through per-level lists of its rows sorted by value, never histogrammed.  values[r] is
+ * row r's value, NaN = missing; the engine stores a missing value as `na_replacement` (the column mean the exact
+ * splitter imputes, training.cc:2385-2392) and -0.0 as +0.0.  A split on it has condition_type YGG_FEATURE_NUMERICAL,
+ * threshold_bin = -1 and threshold_value = the float threshold: value >= threshold_value goes to the positive child,
+ * na_value = na_replacement >= threshold_value.  The feature becomes YGG_FEATURE_NUMERICAL and its byte column a
+ * one-bucket filler.  INVALID_ARGUMENT for +-inf values, a non-finite na_replacement, a wrong row count, a categorical,
+ * wide or already numerical feature, or a call after ygg_gbt_create on the dataset.  Single GPU only (the shard setters
+ * return YGG_ERR_UNIMPLEMENTED); validation / prediction datasets must have the same numerical features. */
+int ygg_dataset_set_numerical_column(ygg_dataset* ds, int32_t feature, const float* values, int64_t n, float na_replacement);
+/* Read-back of a presorted numerical column as stored: values[n_rows] (missing values replaced). */
+int ygg_dataset_get_numerical_column(const ygg_dataset* ds, int32_t feature, float* values);
 int ygg_dataset_destroy(ygg_dataset* ds);
 int64_t ygg_dataset_num_rows(const ygg_dataset* ds);
 int32_t ygg_dataset_num_features(const ygg_dataset* ds);
@@ -420,14 +435,16 @@ int ygg_debug_wide_histogram(ygg_gbt* h, int32_t n_slots, uint64_t* out_sum, uin
 
 /* SplitExamplesInPlace seam (learner/decision_tree/training.cc:5243-5305 ->
  * model/decision_tree/decision_tree.cc:957-1012): stable two-way partition of a row-id list by
- * `bin(feature,row) >= threshold_bin`; positives then negatives, both ascending-stable.
+ * `bin(feature,row) >= threshold_bin`; positives then negatives, both ascending-stable.  YGG_ERR_UNIMPLEMENTED on a
+ * presorted numerical feature (it has no bins).
  * rows_in/rows_out are host pointers of n entries; *n_pos receives the positive count. */
 int ygg_partition_rows(ygg_dataset* ds, const uint32_t* rows_in, int64_t n, int32_t feature,
                        int32_t threshold_bin, uint32_t* rows_out, int64_t* n_pos);
 
 /* Per-kernel device time of the last ygg_gbt_step/train call, in milliseconds, summed over
  * launches, measured with CUDA events on the handle's stream when profiling is enabled.
- * names: "grad", "hist", "scan", "select", "partition", "total". */
+ * names: "grad", "hist", "scan", "select", "partition", "total"; with presorted numerical columns also "presort_scan"
+ * (their scan, included in "scan") and "presort_partition" (their list partition, after "partition"). */
 int ygg_gbt_set_profiling(ygg_gbt* h, int32_t enabled);
 int ygg_gbt_get_profile(ygg_gbt* h, const char* name, double* ms, int64_t* launches);
 

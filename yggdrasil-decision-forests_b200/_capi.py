@@ -42,6 +42,7 @@ assert NODE_DTYPE.itemsize == 112  # sizeof(ygg_node), include/ygg_b200.h
 
 FEATURE_DISCRETIZED_NUMERICAL = 0
 FEATURE_CATEGORICAL = 1
+FEATURE_NUMERICAL = 2   # presorted numerical column (Dataset.set_numerical_column)
 
 HIST_ROOT_SUM, HIST_PACKED, HIST_SHARED, HIST2 = 0, 1, 2, 3   # enum ygg_hist_mode
 
@@ -79,6 +80,7 @@ EXPORTS = [
     "ygg_comm_unique_id", "ygg_comm_create", "ygg_comm_destroy", "ygg_comm_allreduce", "ygg_comm_allgather", "ygg_comm_reducescatter",
     "ygg_dataset_set_wide_column", "ygg_dataset_get_wide_column", "ygg_debug_wide_histogram",
     "ygg_dataset_set_wide_categorical_column", "ygg_gbt_get_category_set",
+    "ygg_dataset_set_numerical_column", "ygg_dataset_get_numerical_column",
 ]
 
 
@@ -184,8 +186,28 @@ class Dataset:
         check(lib().ygg_dataset_get_wide_column(self.handle, C.c_int32(int(feature)), ptr(out, C.c_uint16), C.byref(nb), C.byref(na)))
         return out, nb.value, na.value
 
+    def set_numerical_column(self, feature, values, na_replacement):
+        """Presorted numerical column: values[r] = the float value of row r (NaN = missing, stored as na_replacement, the
+        column mean).  Split by the exact numerical splitter through sorted row lists, with no limit on distinct values;
+        its splits route by value >= threshold_value."""
+        v = np.ascontiguousarray(values, dtype=np.float32)
+        check(lib().ygg_dataset_set_numerical_column(self.handle, C.c_int32(int(feature)), ptr(v, C.c_float), C.c_int64(len(v)),
+                                                     C.c_float(float(np.float32(na_replacement)))))
+        self.num_bins = self.num_bins.copy()
+        self.na_bin = self.na_bin.copy()
+        self.num_bins[feature], self.na_bin[feature] = 1, 0   # the byte column is a one-bucket filler
+        self.feature_types = self.feature_types.copy()
+        self.feature_types[feature] = FEATURE_NUMERICAL
+
+    def get_numerical_column(self, feature):
+        """-> float32 values of a presorted numerical column as stored (missing values replaced)."""
+        out = np.empty(self.n_rows, np.float32)
+        check(lib().ygg_dataset_get_numerical_column(self.handle, C.c_int32(int(feature)), ptr(out, C.c_float)))
+        return out
+
     def set_feature_types(self, feature_types):
-        """feature_types[f]: FEATURE_DISCRETIZED_NUMERICAL or FEATURE_CATEGORICAL."""
+        """feature_types[f]: FEATURE_DISCRETIZED_NUMERICAL or FEATURE_CATEGORICAL (FEATURE_NUMERICAL, and only that, for
+        the presorted numerical columns)."""
         ft = np.ascontiguousarray(feature_types, dtype=np.int32)
         check(lib().ygg_dataset_set_feature_types(self.handle, ptr(ft, C.c_int32), C.c_int32(len(ft))))
         self.feature_types = ft

@@ -22,6 +22,7 @@
 
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <nvtx3/nvToolsExt.h>   // header-only: the ranges cost nothing unless a profiler injects itself
 
 #include "../../include/ygg_b200.h"
@@ -29,6 +30,7 @@
 #include "../../include/ygg_b200_model.h"
 #include "ygg_kernels.cuh"
 #include "ygg_wide.cuh"
+#include "ygg_presort.cuh"
 
 using namespace ygg;
 
@@ -190,6 +192,22 @@ struct ygg_gbt {
   double* d_sort_key = nullptr;
   int32_t* d_sort_idx = nullptr;
   uint32_t* d_sets = nullptr;
+  // presorted numerical columns (DESIGN.md §22): the master lists [P][n] of (value, row) sorted by value, the two level
+  // lists (ping-pong), the scan's prefix sums [P][n] (the first also holds the partition's flags), the segment starts
+  // [max_nodes] and lengths [levels], the best score / boundary per (level node, column), cub's scratch
+  float* d_master_val = nullptr;
+  uint32_t* d_master_row = nullptr;
+  float* d_list_val[2] = {nullptr, nullptr};
+  uint32_t* d_list_row[2] = {nullptr, nullptr};
+  unsigned long long* d_ps = nullptr;
+  unsigned long long* d_ph = nullptr;
+  int64_t* d_seg_off = nullptr;
+  int64_t* d_seg_total = nullptr;
+  unsigned long long* d_sbest = nullptr;
+  unsigned long long* d_sbest_idx = nullptr;
+  int32_t* d_num_feature = nullptr;
+  void* d_presort_temp = nullptr;
+  size_t presort_temp_bytes = 0;
   bool scratch_tree = false;         // d_nodes_scratch holds the tree of the last ygg_tree_train_on_gradients call
   ShardBest* d_shard_best = nullptr;
   TieRec* d_ties = nullptr;        // [max level nodes] ties of the level being selected (single GPU)
@@ -645,12 +663,15 @@ int allocate_wide_buffers(ygg_gbt* h) {
   h->sort_total = 0;
   h->wide_total = 0;
   h->wide_slots = 0;
-  if (ds->n_wide() == 0 || h->num_levels == 0) return YGG_OK;
+  if ((ds->n_wide() == 0 && ds->n_num() == 0) || h->num_levels == 0) return YGG_OK;
   YGG_CUDA(cudaDeviceSynchronize());   // the freed planes go back to the pool before the new ones are taken
   const int f_scan = h->f_end - h->f_begin;
+  const size_t nodes = static_cast<size_t>(1) << std::max(0, h->num_levels - 1);
+  // the float thresholds of the wide and the presorted numerical candidates
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_thr, nodes * f_scan));
+  if (ds->n_wide() == 0) return YGG_OK;
   h->wide_total = ds->wide_off.back();
   h->wide_slots = level_slot_bound(h, h->num_levels - 1);
-  const size_t nodes = static_cast<size_t>(1) << std::max(0, h->num_levels - 1);
   const bool hh = hist_hess(h);
   const size_t per_bucket = sizeof(unsigned long long) + sizeof(uint32_t) + (hh ? sizeof(unsigned long long) : 0);
   const size_t slot_elems = static_cast<size_t>(h->wide_slots) * h->wide_total, node_elems = nodes * h->wide_total;
@@ -668,7 +689,6 @@ int allocate_wide_buffers(ygg_gbt* h) {
     if (dev_alloc(&h->d_wnode_sum[i], node_elems) != YGG_OK || dev_alloc(&h->d_wnode_cnt[i], node_elems) != YGG_OK ||
         (hh && dev_alloc(&h->d_wnode_hsum[i], node_elems) != YGG_OK))
       return fail();
-  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_thr, nodes * f_scan));
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_feature, ds->n_wide()));
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_bins, ds->n_wide()));
   YGG_CUDA(cudaMemcpy(h->d_wide_feature, ds->wide_feature.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
@@ -730,6 +750,126 @@ int accumulate_wide(ygg_gbt* h, int slots) {
   k_hist_wide<<<grid, 256, 0, h->stream>>>(wp);
   h->launches_total++;
   return check_launch("k_hist_wide");
+}
+
+int elementwise_grid(const ygg_gbt* h) { return h->ds->num_sms * 8; }
+
+__global__ void k_iota(uint32_t* out, int64_t n) {
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = static_cast<uint32_t>(i);
+}
+
+// Presorted numerical columns (DESIGN.md §22), once per training handle: per column and row 8 B of master list, 2 x 8 B of
+// level lists and 16 B of prefix sums, plus cub's scratch; then the master lists, sorted by value with ties in row order
+// (a stable radix sort of the rows in order).  A failed allocation is reported with the size it asked for.
+int allocate_presort_buffers(ygg_gbt* h) {
+  const ygg_dataset* ds = h->ds;
+  const int P = ds->n_num();
+  if (P == 0 || h->num_levels == 0) return YGG_OK;
+  const int64_t n = ds->n;
+  const int64_t total = static_cast<int64_t>(P) * n;
+  const size_t nodes = static_cast<size_t>(1) << std::max(0, h->num_levels - 1);
+  size_t sort_bytes = 0, sum_bytes = 0, flag_bytes = 0;
+  YGG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, static_cast<const float*>(nullptr), static_cast<float*>(nullptr),
+                                           static_cast<const uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr), static_cast<int>(n)));
+  YGG_CUDA(cub::DeviceScan::InclusiveSum(nullptr, sum_bytes, static_cast<unsigned long long*>(nullptr),
+                                         static_cast<unsigned long long*>(nullptr), total));
+  YGG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, flag_bytes, static_cast<uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr), total));
+  h->presort_temp_bytes = std::max({sort_bytes, sum_bytes, flag_bytes});
+  bool ok = dev_alloc(&h->d_master_val, total) == YGG_OK && dev_alloc(&h->d_master_row, total) == YGG_OK &&
+            dev_alloc(&h->d_ps, total) == YGG_OK && dev_alloc(&h->d_ph, total) == YGG_OK &&
+            dev_alloc(reinterpret_cast<char**>(&h->d_presort_temp), h->presort_temp_bytes) == YGG_OK;
+  for (int i = 0; i < 2 && ok; i++) ok = dev_alloc(&h->d_list_val[i], total) == YGG_OK && dev_alloc(&h->d_list_row[i], total) == YGG_OK;
+  if (!ok) {
+    (void)cudaGetLastError();
+    return set_error(YGG_ERR_CUDA, "presorted numerical columns: %.2f GB of sorted lists and prefix sums (%d columns x %lld rows x 40 B "
+                     "+ %.2f GB of scan scratch) could not be allocated", (static_cast<double>(total) * 40 + h->presort_temp_bytes) / 1e9,
+                     P, static_cast<long long>(n), static_cast<double>(h->presort_temp_bytes) / 1e9);
+  }
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_seg_off, h->max_nodes));
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_seg_total, 32));
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_sbest, nodes * P));
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_sbest_idx, nodes * P));
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_num_feature, P));
+  YGG_CUDA(cudaMemcpy(h->d_num_feature, ds->num_feature.data(), sizeof(int32_t) * P, cudaMemcpyHostToDevice));
+  k_iota<<<elementwise_grid(h), 256, 0, h->stream>>>(h->d_list_row[0], n);
+  YGG_RETURN_IF_ERROR(check_launch("k_iota"));
+  for (int p = 0; p < P; p++)
+    YGG_CUDA(cub::DeviceRadixSort::SortPairs(h->d_presort_temp, h->presort_temp_bytes, ds->d_num + static_cast<int64_t>(p) * ds->n_pad,
+                                             h->d_master_val + static_cast<int64_t>(p) * n, h->d_list_row[0],
+                                             h->d_master_row + static_cast<int64_t>(p) * n, static_cast<int>(n), 0, 32, h->stream));
+  YGG_CUDA(cudaStreamSynchronize(h->stream));
+  return YGG_OK;
+}
+
+// The presorted columns' parameters of level l: its lists are the master lists at an unsampled root, else the level
+// buffer of its parity (a sampled root is compacted into buffer 0; level l's partition writes buffer (l + 1) & 1).
+PresortParams presort_params(ygg_gbt* h, NodeRec* nodes, int l, const ScanParams& sc) {
+  const ygg_dataset* ds = h->ds;
+  PresortParams p{};
+  p.s = sc; p.level = l; p.P = ds->n_num(); p.n = ds->n; p.num_feature = h->d_num_feature;
+  const bool master = l == 0 && !sampling(h);
+  p.val = master ? h->d_master_val : h->d_list_val[l & 1];
+  p.row = master ? h->d_master_row : h->d_list_row[l & 1];
+  p.s.nodes = nodes; p.s.levels = h->d_levels;
+  p.node_of_row = h->d_node_of_row; p.seg_off = h->d_seg_off; p.seg_total = h->d_seg_total;
+  p.q24 = h->d_q24; p.hq24 = hist_hess(h) ? h->d_hq24 : nullptr; p.ps = h->d_ps; p.ph = h->d_ph;
+  p.best = h->d_sbest; p.best_idx = h->d_sbest_idx; p.thr_value = h->d_wide_thr;
+  return p;
+}
+
+// The scan of level l's presorted lists (after k_scan): the root's segments (and, sampled, its compacted lists), the
+// prefix sums of the lists' quantised gradients, the two boundary passes and the candidates.
+int presort_scan(ygg_gbt* h, const PresortParams& p) {
+  const int64_t total = static_cast<int64_t>(p.P) * p.n;
+  const int grid = elementwise_grid(h);
+  if (p.level == 0) {
+    k_presort_segments<<<1, 1024, 0, h->stream>>>(h->d_levels, p.s.nodes, 0, h->d_seg_off, h->d_seg_total);
+    h->launches_total++;
+    YGG_RETURN_IF_ERROR(check_launch("k_presort_segments"));
+    if (sampling(h)) {   // the iteration's sample, once per tree
+      uint32_t* flags = reinterpret_cast<uint32_t*>(h->d_ps);
+      k_presort_sample_flags<<<grid, 256, 0, h->stream>>>(h->d_master_row, total, h->d_selected, flags);
+      YGG_CUDA(cub::DeviceScan::ExclusiveSum(h->d_presort_temp, h->presort_temp_bytes, flags, flags, total, h->stream));
+      k_presort_sample_scatter<<<grid, 256, 0, h->stream>>>(h->d_master_val, h->d_master_row, p.n, total, h->d_selected, flags,
+                                                            h->d_list_val[0], h->d_list_row[0]);
+      h->launches_total += 3;
+      YGG_RETURN_IF_ERROR(check_launch("k_presort_sample_scatter"));
+    }
+  }
+  k_presort_gather<<<grid, 256, 0, h->stream>>>(p);
+  YGG_CUDA(cub::DeviceScan::InclusiveSum(h->d_presort_temp, h->presort_temp_bytes, h->d_ps, h->d_ps, total, h->stream));
+  if (p.hq24 != nullptr)
+    YGG_CUDA(cub::DeviceScan::InclusiveSum(h->d_presort_temp, h->presort_temp_bytes, h->d_ph, h->d_ph, total, h->stream));
+  const size_t slots = (static_cast<size_t>(1) << p.level) * p.P;
+  YGG_CUDA(cudaMemsetAsync(h->d_sbest, 0, slots * sizeof(unsigned long long), h->stream));
+  YGG_CUDA(cudaMemsetAsync(h->d_sbest_idx, 0xFF, slots * sizeof(unsigned long long), h->stream));
+  if (hist_hess(h) || use_hess(h)) {
+    k_presort_scan<true, true><<<grid, 256, 0, h->stream>>>(p);
+    k_presort_scan<true, false><<<grid, 256, 0, h->stream>>>(p);
+  } else {
+    k_presort_scan<false, true><<<grid, 256, 0, h->stream>>>(p);
+    k_presort_scan<false, false><<<grid, 256, 0, h->stream>>>(p);
+  }
+  k_presort_candidates<<<static_cast<unsigned>((slots + 255) / 256), 256, 0, h->stream>>>(p);
+  h->launches_total += 5 + (p.hq24 != nullptr ? 1 : 0);
+  return check_launch("k_presort_candidates");
+}
+
+// After level l's k_partition: the next level's segments, then every list stable-partitioned into its children's
+// segments (flags of the entries going positive, their exclusive scan, the scatter) in the other level buffer.
+int presort_partition(ygg_gbt* h, NodeRec* nodes, int l) {
+  ScanParams sc{};
+  PresortParams p = presort_params(h, nodes, l, sc);
+  const int64_t total = static_cast<int64_t>(p.P) * p.n;
+  const int grid = elementwise_grid(h);
+  k_presort_segments<<<1, 1024, 0, h->stream>>>(h->d_levels, nodes, l + 1, h->d_seg_off, h->d_seg_total);
+  uint32_t* flags = reinterpret_cast<uint32_t*>(h->d_ps);
+  k_presort_flags<<<grid, 256, 0, h->stream>>>(p, flags);
+  YGG_CUDA(cub::DeviceScan::ExclusiveSum(h->d_presort_temp, h->presort_temp_bytes, flags, flags, total, h->stream));
+  k_presort_scatter<<<grid, 256, 0, h->stream>>>(p, flags, h->d_list_val[(l + 1) & 1], h->d_list_row[(l + 1) & 1]);
+  h->launches_total += 4;
+  return check_launch("k_presort_scatter");
 }
 
 // (Re)allocates everything whose size depends on the feature shard.
@@ -861,8 +1001,6 @@ int accumulate_level(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* lev
   }
   return launch_hist(h, hp, pl.mode, pl.grid, smem);
 }
-
-int elementwise_grid(const ygg_gbt* h) { return h->ds->num_sms * 8; }
 
 int do_allreduce(ygg_gbt* h, void* buf, int64_t count, int dtype, int op) {
   if (h->allreduce == nullptr) return set_error(YGG_ERR_INVALID_ARGUMENT, "row sharding without an all-reduce function");
@@ -1035,6 +1173,10 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
           YGG_RETURN_IF_ERROR(check_launch("k_scan_wide_cat"));
         }
       }
+      if (ds->n_num() > 0) {   // after k_scan: overwrites its (never found) candidates of the presorted features
+        ProfScope psp(h, "presort_scan");
+        YGG_RETURN_IF_ERROR(presort_scan(h, presort_params(h, nodes, l, sc)));
+      }
     }
     {
       ProfScope ps(h, "select");
@@ -1052,7 +1194,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       sel.max_depth = h->cfg.max_depth; sel.sibling_subtraction = h->cfg.sibling_subtraction;
       sel.max_slots = (l + 1 < h->num_levels) ? level_slot_bound(h, l + 1) : 0x7fffffff;
       sel.st = h->d_st; sel.max_nodes = h->max_nodes;
-      sel.wide_of = h->wide_total > 0 ? ds->d_wide_of : nullptr; sel.wide_thr_value = h->wide_total > 0 ? h->d_wide_thr : nullptr;
+      sel.wide_of = h->wide_total > 0 ? ds->d_wide_of : nullptr; sel.wide_thr_value = h->d_wide_thr;
       sel.wide_set = h->d_wide_set; sel.wide_na_bin = h->d_wide_na_bin; sel.n_wide = ds->n_wide(); sel.set_words = h->set_words;
       const int threads = 256, blocks = (level_nodes_bound + (threads / 32) - 1) / (threads / 32);
       k_select_local<<<blocks, threads, 0, h->stream>>>(sel);
@@ -1109,8 +1251,9 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       const bool any_cat = std::any_of(ds->feature_type.begin(), ds->feature_type.end(),
                                        [](int32_t t) { return t == YGG_FEATURE_CATEGORICAL; });
       const int pgrid = (h->n_blocks + per_cta - 1) / per_cta;
-      if (ds->n_wide() > 0) {   // the byte-only instantiations stay as they are for datasets without wide columns
+      if (ds->n_wide() > 0 || ds->n_num() > 0) {   // the byte-only instantiations stay as they are for datasets without them
         pp.wide = ds->d_wide; pp.wide_of = ds->d_wide_of; pp.sets = sets_of(h, nodes); pp.set_words = h->set_words;
+        pp.num = ds->d_num; pp.num_of = ds->d_num_of;
         if (any_cat) k_partition_wide<true><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
         else k_partition_wide<false><<<pgrid, kPartThreads, smem, h->stream>>>(pp);
       } else if (any_cat) {
@@ -1121,6 +1264,10 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       h->launches_total++;
       YGG_RETURN_IF_ERROR(check_launch("k_partition"));
       if (l + 1 < h->num_levels) YGG_RETURN_IF_ERROR(replicate_stats(h, lbn, children_bound));
+    }
+    if (ds->n_num() > 0 && l + 1 < h->num_levels) {
+      ProfScope ps(h, "presort_partition");
+      YGG_RETURN_IF_ERROR(presort_partition(h, nodes, l));
     }
     if (l + 1 == h->num_levels) {
       // last level: its children are leaves; reduce their statistics alone and finish them
@@ -1136,7 +1283,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
     // which of the tied candidates recorded by k_select_local cut their node's rows exactly like the chosen split
     ProfScope ps(h, "select");
     k_verify_ties<<<elementwise_grid(h), 256, 0, h->stream>>>(nodes, h->d_node_of_row, ds->d_bins, ds->n, ds->n_pad, ds->d_wide,
-                                                              ds->n_wide() > 0 ? ds->d_wide_of : nullptr);
+                                                              ds->n_wide() > 0 ? ds->d_wide_of : nullptr, ds->d_num, ds->d_num_of);
     h->launches_total++;
     YGG_RETURN_IF_ERROR(check_launch("k_verify_ties"));
   }
@@ -1266,16 +1413,23 @@ __global__ void __launch_bounds__(256) k_apply_leaves(float* __restrict__ pred, 
 // Validation rows: UpdatePredictions on the held-out rows by tree traversal (loss_utils.cc:214-229,
 // gradient_boosted_trees.cc:1556-1566) fused with the validation loss of the iteration
 // (:1610-1626; loss_imp_binomial.cc:204-234, metric/metric.cc:2173-2199).
-// The bucket of row r of feature f: its uint16 code for a wide column (`wide_of` null: the dataset has none), else its byte.
+// The bucket of row r for split node nd on feature f: value >= nd.thr_value (0 or 1; such splits have thr = 1) for a
+// presorted numerical column, its uint16 code for a wide column (`wide_of` / `num_of` null: the dataset has none), else
+// its byte.
 __device__ __forceinline__ uint32_t row_bin(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
-                                            const int32_t* __restrict__ wide_of, int64_t n_pad, int f, int64_t r) {
+                                            const int32_t* __restrict__ wide_of, const float* __restrict__ num,
+                                            const int32_t* __restrict__ num_of, int64_t n_pad, const NodeRec& nd, int64_t r) {
+  const int f = nd.feature;
+  const int ni = num_of != nullptr ? num_of[f] : -1;
+  if (ni >= 0) return num[static_cast<int64_t>(ni) * n_pad + r] >= nd.thr_value ? 1u : 0u;
   const int wi = wide_of != nullptr ? wide_of[f] : -1;
   return wi >= 0 ? wide[static_cast<int64_t>(wi) * n_pad + r] : bins[static_cast<int64_t>(f) * n_pad + r];
 }
 
 template <int LOSS>
 __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
-                                                      const int32_t* __restrict__ wide_of, int64_t n, int64_t n_pad,
+                                                      const int32_t* __restrict__ wide_of, const float* __restrict__ num,
+                                                      const int32_t* __restrict__ num_of, int64_t n, int64_t n_pad,
                                                       const NodeRec* __restrict__ tree, const uint32_t* __restrict__ sets,
                                                       int set_words, float* __restrict__ pred,
                                                       const uint8_t* __restrict__ label_u8,
@@ -1289,7 +1443,7 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
     while (true) {
       const int f = tree[node].feature;
       if (f < 0) break;
-      const uint32_t b = row_bin(bins, wide, wide_of, n_pad, f, r);
+      const uint32_t b = row_bin(bins, wide, wide_of, num, num_of, n_pad, tree[node], r);
       const bool wide_split = wide_of != nullptr && wide_of[f] >= 0;
       const bool pos = split_goes_pos(tree[node], b, wide_split, sets + static_cast<size_t>(node) * set_words);
       node = pos ? tree[node].pos_child : tree[node].neg_child;
@@ -1331,7 +1485,8 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
 // gradient_boosted_trees.cc:2872-2930: the predictions a resumed training starts from): initial prediction + the leaves
 // reached in every tree of the row's class plane.  One thread per row, trees in order (float sums in the reference's order).
 __global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
-                                                const int32_t* __restrict__ wide_of, int64_t n, int64_t n_pad, const NodeRec* __restrict__ trees,
+                                                const int32_t* __restrict__ wide_of, const float* __restrict__ num,
+                                                const int32_t* __restrict__ num_of, int64_t n, int64_t n_pad, const NodeRec* __restrict__ trees,
                                                 const uint32_t* __restrict__ sets, int set_words, int pool_nodes, int max_nodes, int n_trees, int K,
                                                 float initial, float* __restrict__ out /*[K][n]*/) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
@@ -1344,7 +1499,7 @@ __global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bin
         while (true) {
           const int f = tree[node].feature;
           if (f < 0) break;
-          const uint32_t b = row_bin(bins, wide, wide_of, n_pad, f, r);
+          const uint32_t b = row_bin(bins, wide, wide_of, num, num_of, n_pad, tree[node], r);
           const bool wide_split = wide_of != nullptr && wide_of[f] >= 0;
           const bool pos = split_goes_pos(tree[node], b, wide_split,
                                           sets + (static_cast<size_t>(t) * pool_nodes + node) * set_words);
@@ -1365,7 +1520,7 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
   const int64_t nv = h->vds->n;
   const int grid = static_cast<int>(std::min<int64_t>((nv + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 8));
   if (is_multinomial(h)) {
-    k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred + static_cast<int64_t>(plane) * nv,
+    k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred + static_cast<int64_t>(plane) * nv,
                                                    nullptr, nullptr, nullptr, nullptr, nullptr, 0.f);
     h->launches_total++;
     YGG_RETURN_IF_ERROR(check_launch("k_valid_update"));
@@ -1382,11 +1537,11 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
     return YGG_OK;
   }
   if (h->cfg.loss == YGG_LOSS_BINOMIAL_LOG_LIKELIHOOD)
-    k_valid_update<0><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
+    k_valid_update<0><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
                                                    h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
                                                    h->d_vweight, h->v_correct_scale);
   else
-    k_valid_update<1><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
+    k_valid_update<1><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
                                                    h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
                                                    h->d_vweight, h->v_correct_scale);
   h->launches_total++;
@@ -1758,6 +1913,10 @@ void preorder(const std::vector<NodeRec>& nodes, int idx, std::vector<ygg_node>*
   o.num_pos_examples = leaf ? 0 : n.n_pos;
   o.stat[0] = n.stat[0]; o.stat[1] = n.stat[1]; o.stat[2] = n.stat[2];
   o.threshold_value = leaf ? std::numeric_limits<float>::quiet_NaN() : n.thr_value;
+  if (!leaf && n.cond_type == YGG_FEATURE_NUMERICAL) {   // (thr = 1 is the engine's bin rule, see k_presort_candidates)
+    o.condition_type = YGG_FEATURE_NUMERICAL;
+    o.threshold_bin = -1;
+  }
   if (!leaf && n.cond_type == YGG_FEATURE_CATEGORICAL) {
     o.condition_type = YGG_FEATURE_CATEGORICAL;
     o.threshold_bin = 0;
@@ -1894,9 +2053,14 @@ int ygg_dataset_create(ygg_dataset** out, int64_t n_rows, int32_t n_features, co
 int ygg_dataset_set_feature_types(ygg_dataset* ds, const int32_t* feature_types, int32_t n_features) {
   if (!ds || !feature_types) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (n_features != ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "n_features=%d, dataset has %d", n_features, ds->F);
-  for (int f = 0; f < n_features; f++)
-    if (feature_types[f] != YGG_FEATURE_DISCRETIZED_NUMERICAL && feature_types[f] != YGG_FEATURE_CATEGORICAL)
-      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: unknown feature type %d", f, feature_types[f]);
+  for (int f = 0; f < n_features; f++) {
+    // (YGG_FEATURE_NUMERICAL is what ygg_dataset_set_numerical_column made of a feature, and stays so)
+    const bool presorted = !ds->num_of.empty() && ds->num_of[f] >= 0;
+    if (presorted ? feature_types[f] != YGG_FEATURE_NUMERICAL
+                  : (feature_types[f] != YGG_FEATURE_DISCRETIZED_NUMERICAL && feature_types[f] != YGG_FEATURE_CATEGORICAL))
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: feature type %d (presorted numerical columns are set with "
+                       "ygg_dataset_set_numerical_column)", f, feature_types[f]);
+  }
   YGG_CUDA(cudaSetDevice(ds->device));
   ds->feature_type.assign(feature_types, feature_types + n_features);
   YGG_CUDA(cudaMemcpy(ds->d_feature_type, feature_types, sizeof(int32_t) * n_features, cudaMemcpyHostToDevice));
@@ -1948,6 +2112,20 @@ int ensure_exact_arrays(ygg_dataset* ds) {
 }  // namespace
 
 namespace {
+// The byte column of a feature held elsewhere (wide or presorted): a filler over all 256 bins with one bucket, i.e. never
+// a valid split for k_scan.  (All rows in one bin would be as good for the scan, but would push k_hist's packed layout,
+// whose bins take at most 8191 rows per work item, to its slower carry layout.)
+int set_filler_column(ygg_dataset* ds, int32_t feature) {
+  std::vector<uint8_t> filler(ds->n);
+  for (int64_t r = 0; r < ds->n; r++) filler[r] = static_cast<uint8_t>(r & 0xFF);
+  YGG_CUDA(cudaMemcpy(ds->d_bins + static_cast<int64_t>(feature) * ds->n_pad, filler.data(), ds->n, cudaMemcpyHostToDevice));
+  dev_free(ds->d_bins4);   // k_hist2's interleaved copy is rebuilt on first use
+  ds->d_bins4 = nullptr;
+  ds->num_bins[feature] = 1;
+  ds->na_bin[feature] = 0;
+  return ygg_internal_dataset_finalize(ds);
+}
+
 // The dataset checks and the upload shared by the wide numerical and the wide categorical columns (`values` null:
 // categorical; its bucket values are zeros).
 int attach_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
@@ -1957,6 +2135,7 @@ int attach_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, 
   if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
   if (ds->handles > 0)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "wide columns are set before ygg_gbt_create: %d handle(s) already use this dataset", ds->handles);
+  if (!ds->num_of.empty() && ds->num_of[feature] >= 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is a presorted numerical column", feature);
   if (!categorical && ds->feature_type[feature] != YGG_FEATURE_DISCRETIZED_NUMERICAL)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is categorical: use ygg_dataset_set_wide_categorical_column", feature);
   if (categorical && ds->feature_type[feature] != YGG_FEATURE_CATEGORICAL)
@@ -1973,17 +2152,7 @@ int attach_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, 
   YGG_CUDA(cudaMemcpy(grown + static_cast<size_t>(W) * ds->n_pad, codes, sizeof(uint16_t) * n, cudaMemcpyHostToDevice));
   dev_free(ds->d_wide);
   ds->d_wide = grown;
-  // the byte column: a filler over all 256 bins with one bucket, i.e. never a valid split for k_scan.  (All rows in one
-  // bin would be as good for the scan, but would push k_hist's packed layout, whose bins take at most 8191 rows per work
-  // item, to its slower carry layout.)
-  std::vector<uint8_t> filler(n);
-  for (int64_t r = 0; r < n; r++) filler[r] = static_cast<uint8_t>(r & 0xFF);
-  YGG_CUDA(cudaMemcpy(ds->d_bins + static_cast<int64_t>(feature) * ds->n_pad, filler.data(), n, cudaMemcpyHostToDevice));
-  dev_free(ds->d_bins4);   // k_hist2's interleaved copy is rebuilt on first use
-  ds->d_bins4 = nullptr;
-  ds->num_bins[feature] = 1;
-  ds->na_bin[feature] = 0;
-  YGG_RETURN_IF_ERROR(ygg_internal_dataset_finalize(ds));
+  YGG_RETURN_IF_ERROR(set_filler_column(ds, feature));
   if (ds->wide_of.empty()) { ds->wide_of.assign(ds->F, -1); ds->wide_off.assign(1, 0); }
   ds->wide_of[feature] = W;
   ds->wide_feature.push_back(feature);
@@ -2046,10 +2215,63 @@ int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t
   return YGG_OK;
 }
 
+int ygg_dataset_set_numerical_column(ygg_dataset* ds, int32_t feature, const float* values, int64_t n, float na_replacement) {
+  // the checks that need no dataset first (they hold without a device too), then those against the dataset
+  if (!values) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (n < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "negative row count %lld", static_cast<long long>(n));
+  if (!std::isfinite(na_replacement)) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: na_replacement must be finite", feature);
+  for (int64_t r = 0; r < n; r++)
+    if (std::isinf(values[r]))
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: value of row %lld is infinite", feature, static_cast<long long>(r));
+  if (!ds) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
+  if (ds->handles > 0)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "numerical columns are set before ygg_gbt_create: %d handle(s) already use this dataset", ds->handles);
+  if (ds->feature_type[feature] == YGG_FEATURE_CATEGORICAL) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is categorical", feature);
+  if (!ds->wide_of.empty() && ds->wide_of[feature] >= 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is a wide column", feature);
+  if (!ds->num_of.empty() && ds->num_of[feature] >= 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is already a presorted numerical column", feature);
+  if (n != ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "%lld values for a dataset of %lld rows", static_cast<long long>(n), static_cast<long long>(ds->n));
+  YGG_RETURN_IF_ERROR(require_device());
+  YGG_CUDA(cudaSetDevice(ds->device));
+  // missing -> the column mean (training.cc:2385-2392); -0.0 -> +0.0, so that the sort and the conditions see one zero
+  std::vector<float> v(values, values + n);
+  for (float& x : v) x = std::isnan(x) ? na_replacement : (x == 0.f ? 0.f : x);
+  const int P = ds->n_num();
+  float* grown = nullptr;   // the value matrix grows by one plane (the old planes are copied over)
+  YGG_RETURN_IF_ERROR(dev_alloc(&grown, static_cast<size_t>(P + 1) * ds->n_pad));
+  if (P > 0) YGG_CUDA(cudaMemcpy(grown, ds->d_num, sizeof(float) * P * ds->n_pad, cudaMemcpyDeviceToDevice));
+  YGG_CUDA(cudaMemcpy(grown + static_cast<size_t>(P) * ds->n_pad, v.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
+  dev_free(ds->d_num);
+  ds->d_num = grown;
+  ds->feature_type[feature] = YGG_FEATURE_NUMERICAL;
+  YGG_RETURN_IF_ERROR(set_filler_column(ds, feature));   // (uploads the feature type too)
+  if (ds->num_of.empty()) ds->num_of.assign(ds->F, -1);
+  ds->num_of[feature] = P;
+  ds->num_feature.push_back(feature);
+  ds->num_na_replacement.push_back(na_replacement);
+  if (ds->d_num_of == nullptr) YGG_RETURN_IF_ERROR(dev_alloc(&ds->d_num_of, ds->F));
+  YGG_CUDA(cudaMemcpy(ds->d_num_of, ds->num_of.data(), sizeof(int32_t) * ds->F, cudaMemcpyHostToDevice));
+  YGG_RETURN_IF_ERROR(ensure_exact_arrays(ds));   // k_select_* read the NA replacement there
+  const int32_t zero = 0;
+  YGG_CUDA(cudaMemcpy(ds->d_exact_rule + feature, &zero, sizeof(zero), cudaMemcpyHostToDevice));
+  YGG_CUDA(cudaMemcpy(ds->d_na_replacement + feature, &na_replacement, sizeof(float), cudaMemcpyHostToDevice));
+  return YGG_OK;
+}
+
+int ygg_dataset_get_numerical_column(const ygg_dataset* ds, int32_t feature, float* values) {
+  if (!ds || !values) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
+  if (ds->num_of.empty() || ds->num_of[feature] < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d is not a presorted numerical column", feature);
+  YGG_CUDA(cudaSetDevice(ds->device));
+  YGG_CUDA(cudaMemcpy(values, ds->d_num + static_cast<size_t>(ds->num_of[feature]) * ds->n_pad, sizeof(float) * ds->n, cudaMemcpyDeviceToHost));
+  return YGG_OK;
+}
+
 int ygg_dataset_destroy(ygg_dataset* ds) {
   if (!ds) return YGG_OK;
   cudaSetDevice(ds->device);
   dev_free(ds->d_wide); dev_free(ds->d_wide_of); dev_free(ds->d_wide_off); dev_free(ds->d_wide_values);
+  dev_free(ds->d_num); dev_free(ds->d_num_of);
   dev_free(ds->d_bins);
   dev_free(ds->d_bins4);
   dev_free(ds->d_num_bins);
@@ -2223,7 +2445,7 @@ static int init_handle(ygg_gbt* h) {
   if (sampling(h)) YGG_RETURN_IF_ERROR(dev_alloc(&h->d_selected, n_pad));
   YGG_CUDA(cudaMemset(h->d_loss, 0, sizeof(LossRec) * h->tree_capacity));
   YGG_RETURN_IF_ERROR(allocate_level_buffers(h));
-  return YGG_OK;
+  return allocate_presort_buffers(h);
 }
 
 int ygg_gbt_destroy(ygg_gbt* h) {
@@ -2249,6 +2471,9 @@ int ygg_gbt_destroy(ygg_gbt* h) {
   dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins);
   dev_free(h->d_wide_cat); dev_free(h->d_wide_na_bin); dev_free(h->d_wide_set); dev_free(h->d_sort_key); dev_free(h->d_sort_idx);
   dev_free(h->d_sets); dev_free(h->d_sort_off);
+  dev_free(h->d_master_val); dev_free(h->d_master_row); dev_free(h->d_ps); dev_free(h->d_ph); dev_free(h->d_presort_temp);
+  for (int i = 0; i < 2; i++) { dev_free(h->d_list_val[i]); dev_free(h->d_list_row[i]); }
+  dev_free(h->d_seg_off); dev_free(h->d_seg_total); dev_free(h->d_sbest); dev_free(h->d_sbest_idx); dev_free(h->d_num_feature);
   cudaFree(h->d_goss_temp);
   cudaFree(h->d_level_buf);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -2445,6 +2670,7 @@ int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature
                               int32_t world, ygg_allgather_fn exchange, void* ctx) {
   if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
   if (h->ds->n_wide() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "wide columns (ygg_dataset_set_wide_column) are single GPU: not combined with feature shards");
+  if (h->ds->n_num() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "presorted numerical columns (ygg_dataset_set_numerical_column) are single GPU: not combined with feature shards");
   if (feature_begin < 0 || feature_end > h->ds->F || feature_begin >= feature_end)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "bad feature shard [%d, %d) of %d", feature_begin, feature_end, h->ds->F);
   if (world < 1 || rank < 0 || rank >= world) return set_error(YGG_ERR_INVALID_ARGUMENT, "bad rank %d / world %d", rank, world);
@@ -2468,6 +2694,7 @@ int ygg_gbt_set_row_shard(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_row
                           float initial_prediction, ygg_allreduce_fn allreduce, void* ctx) {
   if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
   if (h->ds->n_wide() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "wide columns (ygg_dataset_set_wide_column) are single GPU: not combined with row shards");
+  if (h->ds->n_num() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "presorted numerical columns (ygg_dataset_set_numerical_column) are single GPU: not combined with row shards");
   if (world < 1 || rank < 0 || rank >= world) return set_error(YGG_ERR_INVALID_ARGUMENT, "bad rank %d / world %d", rank, world);
   if (world > 1 && !allreduce) return set_error(YGG_ERR_INVALID_ARGUMENT, "world > 1 needs an all-reduce function");
   if (n_rows_global < h->ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "n_rows_global < local rows");
@@ -2507,6 +2734,7 @@ int ygg_gbt_set_row_shard_scatter(ygg_gbt* h, int32_t rank, int32_t world, int64
                                   ygg_reducescatter_fn reducescatter, ygg_allgather_fn allgather, void* ctx) {
   if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
   if (h->ds->n_wide() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "wide columns (ygg_dataset_set_wide_column) are single GPU: not combined with row shards");
+  if (h->ds->n_num() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "presorted numerical columns (ygg_dataset_set_numerical_column) are single GPU: not combined with row shards");
   if (world > 1 && (!reducescatter || !allgather)) return set_error(YGG_ERR_INVALID_ARGUMENT, "world > 1 needs reduce-scatter and all-gather functions");
   if (world > h->ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "more ranks (%d) than features (%d)", world, h->ds->F);
   YGG_RETURN_IF_ERROR(ygg_gbt_set_row_shard(h, rank, world, n_rows_global, initial_prediction, allreduce, ctx));
@@ -2532,6 +2760,14 @@ int ygg_gbt_set_row_shard_scatter(ygg_gbt* h, int32_t rank, int32_t world, int64
 namespace {
 __global__ void k_gather_rows(const uint8_t* __restrict__ in, int64_t in_pad, const uint32_t* __restrict__ rows, int64_t n_out,
                               int64_t out_pad, uint8_t* __restrict__ out) {
+  const int f = blockIdx.y;
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_out; i += stride)
+    out[static_cast<int64_t>(f) * out_pad + i] = in[static_cast<int64_t>(f) * in_pad + rows[i]];
+}
+// the same for the presorted numerical columns' float planes
+__global__ void k_gather_rows32(const float* __restrict__ in, int64_t in_pad, const uint32_t* __restrict__ rows, int64_t n_out,
+                                int64_t out_pad, float* __restrict__ out) {
   const int f = blockIdx.y;
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_out; i += stride)
@@ -2614,6 +2850,18 @@ int ygg_dataset_split_rows(const ygg_dataset* ds, const uint8_t* select, ygg_dat
       if (st == YGG_OK) {
         dim3 wgrid(grid.x, static_cast<unsigned>(ds->n_wide()));
         k_gather_rows16<<<wgrid, 256>>>(ds->d_wide, ds->n_pad, d_rows, n, o->n_pad, o->d_wide);
+      }
+    }
+    if (st == YGG_OK && ds->n_num() > 0) {   // the presorted columns travel with the rows: values and NA replacements
+      ygg_dataset* o = out[k];
+      o->num_of = ds->num_of; o->num_feature = ds->num_feature; o->num_na_replacement = ds->num_na_replacement;
+      st = dev_alloc(&o->d_num, static_cast<size_t>(ds->n_num()) * o->n_pad);
+      if (st == YGG_OK) st = dev_alloc(&o->d_num_of, ds->F);
+      if (st == YGG_OK && cudaMemcpy(o->d_num_of, ds->num_of.data(), sizeof(int32_t) * ds->F, cudaMemcpyHostToDevice) != cudaSuccess)
+        st = set_error(YGG_ERR_CUDA, "upload of the numerical column table failed");
+      if (st == YGG_OK) {
+        dim3 ngrid(grid.x, static_cast<unsigned>(ds->n_num()));
+        k_gather_rows32<<<ngrid, 256>>>(ds->d_num, ds->n_pad, d_rows, n, o->n_pad, o->d_num);
       }
     }
     if (st == YGG_OK && cudaDeviceSynchronize() != cudaSuccess) st = set_error(YGG_ERR_CUDA, "row gather failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -2977,7 +3225,7 @@ int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   YGG_RETURN_IF_ERROR(dev_alloc(&d_out, static_cast<size_t>(n)));
   const int n_trees = ygg_gbt_num_trees(h);
   k_predict<<<static_cast<int>(std::min<int64_t>((ds->n + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 16)), 256, 0, h->stream>>>(
-      ds->d_bins, ds->d_wide, ds->d_wide_of, ds->n, ds->n_pad, h->d_nodes_all, h->d_sets, h->set_words, pool_nodes(h), h->max_nodes, n_trees, h->K, h->initial_prediction, d_out);
+      ds->d_bins, ds->d_wide, ds->d_wide_of, ds->d_num, ds->d_num_of, ds->n, ds->n_pad, h->d_nodes_all, h->d_sets, h->set_words, pool_nodes(h), h->max_nodes, n_trees, h->K, h->initial_prediction, d_out);
   h->launches_total++;
   int st = check_launch("k_predict");
   if (st == YGG_OK && (cudaMemcpyAsync(out, d_out, sizeof(float) * n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
@@ -3232,6 +3480,8 @@ int ygg_partition_rows(ygg_dataset* ds, const uint32_t* rows_in, int64_t n, int3
                        int32_t threshold_bin, uint32_t* rows_out, int64_t* n_pos) {
   if (!ds || !rows_in || !rows_out || !n_pos) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
+  if (ds->feature_type[feature] == YGG_FEATURE_NUMERICAL)
+    return set_error(YGG_ERR_UNIMPLEMENTED, "feature %d is a presorted numerical column: it has no bins to partition by", feature);
   if (n < 0 || n >= (1ll << 32)) return set_error(YGG_ERR_INVALID_ARGUMENT, "bad row count");
   if (n == 0) { *n_pos = 0; return YGG_OK; }
   for (int64_t i = 0; i < n; i++)

@@ -41,6 +41,14 @@ struct ygg_dataset {
       if (wide_cat[w]) m = std::max(m, (wide_bins[w] + 31) / 32);
     return m;
   }
+  // Presorted numerical columns (ygg_dataset_set_numerical_column, DESIGN.md §22): float values, NaN already replaced by
+  // the column mean and -0.0 stored as +0.0.  feature_type[f] = YGG_FEATURE_NUMERICAL and the byte column is the same
+  // one-bucket filler as a wide column's.
+  float* d_num = nullptr;              // [numerical features][n_pad] values, in numerical-index order
+  int32_t* d_num_of = nullptr;         // [F] numerical index of a feature, -1 otherwise
+  std::vector<int32_t> num_of, num_feature;
+  std::vector<float> num_na_replacement;
+  int n_num() const { return static_cast<int>(num_feature.size()); }
   int handles = 0;                     // live ygg_gbt handles on this dataset (wide columns are set before the first)
 };
 

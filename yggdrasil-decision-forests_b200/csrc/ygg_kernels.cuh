@@ -752,8 +752,9 @@ struct SelectParams {
   int max_slots;               // capacity of one histogram pass
   DeviceState* st;
   int max_nodes;
-  // wide columns (single GPU): the float thresholds k_scan_wide left per (level node, feature); null without wide columns
-  const int32_t* wide_of;      // [F] wide index, -1 for a byte column
+  // wide and presorted numerical columns (single GPU): the float thresholds k_scan_wide / k_presort_candidates left per
+  // (level node, feature); null without such columns
+  const int32_t* wide_of;      // [F] wide index, -1 for a byte column (null without wide columns)
   const float* wide_thr_value; // [level nodes][f_count]
   // wide categorical columns: the positive sets k_scan_wide_cat left per (level node, wide feature) (null without them)
   const uint32_t* wide_set;    // [level nodes][n_wide][set_words]
@@ -769,11 +770,13 @@ __device__ __forceinline__ int wide_cat_index(const SelectParams& p, int fg, int
   return (p.wide_set != nullptr && cond_type == 1) ? p.wide_of[fg] : -1;
 }
 
-// The float threshold of candidate (level node j, local feature fl): a wide column's from k_scan_wide's side array, a
-// lossless byte column's from its packed threshold, NaN for a discretized one.
+// The float threshold of candidate (level node j, local feature fl): a wide or presorted numerical column's from the side
+// array k_scan_wide / k_presort_candidates fill, a lossless byte column's from its packed threshold, NaN for a
+// discretized one.
 __device__ __forceinline__ float candidate_thr_value(const SelectParams& p, int j, int fl, int32_t thr) {
   const int fg = p.f_begin + fl;
-  if (p.wide_thr_value != nullptr && p.wide_of[fg] >= 0) return p.wide_thr_value[static_cast<size_t>(j) * p.f_count + fl];
+  if (p.wide_thr_value != nullptr && ((p.wide_of != nullptr && p.wide_of[fg] >= 0) || p.feature_type[fg] == 2))
+    return p.wide_thr_value[static_cast<size_t>(j) * p.f_count + fl];
   return p.bucket_values != nullptr ? thr_value_of(thr, p.bucket_values + static_cast<size_t>(fg) * kMaxBins) : __builtin_nanf("");
 }
 
@@ -947,7 +950,7 @@ __global__ void __launch_bounds__(256) k_select_global(SelectParams p) {
       if (best.feature >= 0 && best.n_pos > 0 && best.n_pos < nd->n) {
         nd->feature = best.feature;
         // (a wide column's side-array entry is this rank's: wide columns are single GPU)
-        nd->thr_value = best.cond_type == 0 ? candidate_thr_value(p, j, best.feature - p.f_begin, best.thr) : __builtin_nanf("");
+        nd->thr_value = best.cond_type != 1 ? candidate_thr_value(p, j, best.feature - p.f_begin, best.thr) : __builtin_nanf("");
         best.thr = thr_bin_of(best.thr);
         nd->thr = best.thr;
         nd->cond_type = best.cond_type;
@@ -1079,6 +1082,8 @@ struct PartParams {
   const int32_t* wide_of;
   const uint32_t* sets;       // k_partition_wide: the tree's positive-set pool [max_nodes][set_words] (wide categorical splits)
   int set_words;
+  const float* num;           // k_partition_wide: the presorted numerical columns (ygg_dataset.d_num / d_num_of; null without)
+  const int32_t* num_of;
 };
 
 // Shared accumulators per child: cnt, g_lo, g_hi, h_lo, h_hi, g2_lo, g2_hi.
@@ -1128,7 +1133,8 @@ __device__ __forceinline__ PartNode make_part_node(const NodeRec* nodes, const N
 // node being split — g / h / q24 (128-bit loads), the relabel, the statistics of the smaller children and the
 // stable compaction of the rows histogrammed at the next level (block-wide exclusive scan; the list stays in ROW
 // ORDER, which k_hist relies on for conflict-free LDS.U8 reads of its bins tile).
-// WIDE (k_partition_wide, datasets with wide columns only): a split on a wide feature reads its uint16 code.
+// WIDE (k_partition_wide, datasets with wide or presorted columns only): a split on a wide feature reads its uint16 code,
+// one on a presorted numerical feature gets the bin value >= thr_value (its thr is 1).
 template <bool CAT, bool WIDE>
 __device__ __forceinline__ void partition_impl(const PartParams& p) {
   extern __shared__ __align__(16) uint32_t smem[];
@@ -1191,9 +1197,11 @@ __device__ __forceinline__ void partition_impl(const PartParams& p) {
           const int li = node - lv.first_node;
           const int feature = nodes_in_smem ? s_nodes[li].feature : p.nodes[node].feature;
           if (feature >= 0) {
-            const int wi = WIDE ? p.wide_of[feature] : -1;
-            const int32_t bin = wi >= 0 ? static_cast<int32_t>(p.wide[static_cast<int64_t>(wi) * p.n_pad + rh + j])
-                                        : static_cast<int32_t>(p.bins[static_cast<int64_t>(feature) * p.n_pad + rh + j]);
+            const int wi = WIDE && p.wide_of != nullptr ? p.wide_of[feature] : -1;
+            const int ni = WIDE && p.num_of != nullptr ? p.num_of[feature] : -1;
+            const int32_t bin = ni >= 0   ? (p.num[static_cast<int64_t>(ni) * p.n_pad + rh + j] >= p.nodes[node].thr_value ? 1 : 0)
+                                : wi >= 0 ? static_cast<int32_t>(p.wide[static_cast<int64_t>(wi) * p.n_pad + rh + j])
+                                          : static_cast<int32_t>(p.bins[static_cast<int64_t>(feature) * p.n_pad + rh + j]);
             lb[j] = (li << kBinBits) | bin;
             any = true;
           }
@@ -1229,7 +1237,7 @@ __device__ __forceinline__ void partition_impl(const PartParams& p) {
             bool go_pos;
             if (!CAT || pn.thr >= 0) {
               go_pos = static_cast<int>(bin) >= pn.thr;
-            } else if (WIDE && p.wide_of[pn.feature] >= 0) {   // a wide categorical split: its set in the pool
+            } else if (WIDE && p.wide_of != nullptr && p.wide_of[pn.feature] >= 0) {   // a wide categorical split: its set in the pool
               const uint32_t mw = p.sets[static_cast<size_t>(lv.first_node + li) * p.set_words + (bin >> 5)];
               go_pos = ((mw >> (bin & 31)) & 1u) != 0;
             } else {
@@ -1562,11 +1570,12 @@ __global__ void __launch_bounds__(1024) k_weight_sums_finish(WeightSumParams p) 
 // the node to the same side (twin columns); equal float scores and equal positive counts do not prove that.  Every
 // row walks from its leaf to the root; at each ancestor with recorded ties it knows on which side it went and
 // evaluates the alternatives' conditions: a disagreement disqualifies the alternative (n_pos = -1).
-// (`wide` / `wide_of`: the dataset's wide columns, null without them.  A wide categorical alternative is recorded with
-// n_pos = -1 by k_select_local: it is never evaluated here.)
+// (`wide` / `wide_of`: the dataset's wide columns, `num` / `num_of` its presorted numerical columns, null without them.
+// A wide categorical alternative is recorded with n_pos = -1 by k_select_local: it is never evaluated here.)
 __global__ void __launch_bounds__(256) k_verify_ties(NodeRec* nodes, const uint16_t* __restrict__ node_of_row,
                                                      const uint8_t* __restrict__ bins, int64_t n, int64_t n_pad,
-                                                     const uint16_t* __restrict__ wide, const int32_t* __restrict__ wide_of) {
+                                                     const uint16_t* __restrict__ wide, const int32_t* __restrict__ wide_of,
+                                                     const float* __restrict__ num, const int32_t* __restrict__ num_of) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n; r += stride) {
     int child = node_of_row[r];
@@ -1579,7 +1588,9 @@ __global__ void __launch_bounds__(256) k_verify_ties(NodeRec* nodes, const uint1
           const TieAlt& a = nodes[node].tie[i];
           if (a.n_pos < 0) continue;
           const int wi = wide_of != nullptr ? wide_of[a.feature] : -1;
-          const uint32_t b = wi >= 0 ? wide[static_cast<int64_t>(wi) * n_pad + r] : bins[static_cast<int64_t>(a.feature) * n_pad + r];
+          const int ni = num_of != nullptr ? num_of[a.feature] : -1;
+          const uint32_t b = ni >= 0   ? (num[static_cast<int64_t>(ni) * n_pad + r] >= a.thr_value ? 1u : 0u)   // (its thr is 1)
+                             : wi >= 0 ? wide[static_cast<int64_t>(wi) * n_pad + r] : bins[static_cast<int64_t>(a.feature) * n_pad + r];
           const bool alt_pos = a.cond_type == 1 ? ((a.mask[b >> 5] >> (b & 31)) & 1u) != 0 : static_cast<int>(b) >= a.thr;
           if (alt_pos != went_pos) nodes[node].tie[i].n_pos = -1;
         }

@@ -88,6 +88,10 @@ std::string encode_node(const ygg_node& n, int use_hessian_gain, const int32_t* 
         cv.bytes(1, packed.s);  // elements, packed
         cond.msg(4, cv);        // contains_condition
       }
+    } else if (n.condition_type == YGG_FEATURE_NUMERICAL) {
+      Pb hi;  // Condition.Higher: value >= threshold (a presorted numerical column)
+      hi.f32(1, n.threshold_value);  // threshold
+      cond.msg(2, hi);               // higher_condition
     } else {
       Pb dh;  // Condition.DiscretizedHigher
       dh.i64(1, n.threshold_bin);

@@ -54,6 +54,26 @@ class DiscretizedColumn:
 
 
 @dataclasses.dataclass
+class PresortedColumn:
+    """A numerical column kept as its float values (_capi.Dataset.set_numerical_column): the exact numerical splitter
+    through sorted row lists, with no limit on distinct values.  Saved as a NUMERICAL column; its splits are Higher
+    conditions (value >= threshold, a missing value takes the node's na_value)."""
+    name: str
+    mean: float               # NA replacement, NumericalSpec.mean
+    min_value: float
+    max_value: float
+    num_missing: int = 0
+    num_values: int = 0
+    num_distinct: int = 0
+    feature_type = _capi.FEATURE_NUMERICAL
+    wide = False
+
+    def encode(self, values) -> np.ndarray:
+        """The float32 values themselves, NaN = missing."""
+        return np.asarray(values, dtype=np.float32)
+
+
+@dataclasses.dataclass
 class CategoricalColumn:
     name: str
     vocabulary: List[str]     # index -> key; vocabulary[0] == "<OOD>"
@@ -203,13 +223,12 @@ def infer_column_lossless(name: str, values, max_rows: Optional[int] = None,
     not in the partition of the training rows."""
     v = np.asarray(values, dtype=np.float32)
     sample = v if (max_rows is None or len(v) <= max_rows) else v[:max_rows]
-    present = sample[~np.isnan(sample)]
     # every row's value must have its own bucket: the distinct set comes from ALL rows, whatever `max_rows` says
     # about the statistics (a value outside the sample would otherwise be merged into a neighbour's bucket)
     distinct = np.unique(v[~np.isnan(v)])
     if len(distinct) == 0 or len(distinct) > max_distinct:   # byte buckets, or wide columns up to max_distinct values
         return None
-    mean = float(present.astype(np.float64).mean()) if len(present) else float(distinct.astype(np.float64).mean())
+    mean = _exact_mean(sample, distinct)
     num_missing = int(np.isnan(v).sum())
     if num_missing > 0:
         # The exact splitter imputes NA with the column mean (training.cc:2385-2392, splitter_scanner.h:1230-1430): the
@@ -227,31 +246,63 @@ def infer_column_lossless(name: str, values, max_rows: Optional[int] = None,
                              num_missing=num_missing, num_values=len(v), bucket_values=distinct.astype(np.float32))
 
 
+def _exact_mean(sample: np.ndarray, distinct: np.ndarray) -> float:
+    """The exact splitter's NA replacement: the mean of the present values of the statistics sample (the first
+    max_num_scanned_rows_to_compute_statistics rows), else of the distinct values of the whole column."""
+    present = sample[~np.isnan(sample)]
+    return float(present.astype(np.float64).mean()) if len(present) else float(distinct.astype(np.float64).mean())
+
+
+def infer_column_presorted(name: str, values, max_rows: Optional[int] = None) -> Optional[PresortedColumn]:
+    """A presorted numerical column (any number of distinct values; None for a column without a present value).  Its
+    mean is infer_column_lossless's, from the same sample."""
+    v = np.asarray(values, dtype=np.float32)
+    sample = v if (max_rows is None or len(v) <= max_rows) else v[:max_rows]
+    distinct = np.unique(v[~np.isnan(v)])
+    if len(distinct) == 0:
+        return None
+    return PresortedColumn(name=name, mean=_exact_mean(sample, distinct), min_value=float(distinct[0]),
+                           max_value=float(distinct[-1]), num_missing=int(np.isnan(v).sum()), num_values=len(v),
+                           num_distinct=len(distinct))
+
+
+def _presorted(c) -> bool:
+    return c.feature_type == _capi.FEATURE_NUMERICAL
+
+
 def encode_features(cols: Dict[str, np.ndarray], columns: Sequence[DiscretizedColumn]) -> np.ndarray:
-    """[features, rows] bucket indices: uint8, or uint16 when a column has more than 256 buckets (wide columns)."""
+    """[features, rows] bucket indices: uint8, or uint16 when a column has more than 256 buckets (wide columns).  With a
+    presorted numerical column the matrix is float64: its rows hold the float32 values (NaN = missing), the others their
+    bucket indices (exact in float64)."""
     n = len(next(iter(cols.values())))
-    wide = any(c.num_bins > 256 for c in columns)
-    out = np.empty((len(columns), n), dtype=np.uint16 if wide else np.uint8)
+    presorted = any(_presorted(c) for c in columns)
+    wide = any(not _presorted(c) and c.num_bins > 256 for c in columns)
+    out = np.empty((len(columns), n), dtype=np.float64 if presorted else (np.uint16 if wide else np.uint8))
     for i, c in enumerate(columns):
-        out[i] = c.encode16(cols[c.name]) if c.num_bins > 256 else c.encode(cols[c.name])
+        out[i] = c.encode(cols[c.name]) if _presorted(c) or c.num_bins <= 256 else c.encode16(cols[c.name])
     return out
 
 
 def device_dataset(bins: np.ndarray, columns: Sequence, device: int = 0) -> "_capi.Dataset":
     """The device dataset of encode_features' output: byte columns as they are, wide columns (more than 256 buckets)
-    attached with their codes (and, numerical, their bucket values and mean)."""
-    wide = [i for i, c in enumerate(columns) if c.num_bins > 256]
+    attached with their codes (and, numerical, their bucket values and mean), presorted numerical columns with their
+    values and mean."""
+    wide = [i for i, c in enumerate(columns) if _presorted(c) or c.num_bins > 256]
     byte_bins = np.zeros(bins.shape, np.uint8) if bins.dtype != np.uint8 else bins
     if bins.dtype != np.uint8:
         narrow = [i for i in range(len(columns)) if i not in set(wide)]
         byte_bins[narrow] = bins[narrow]
     num_bins = [1 if i in wide else c.num_bins for i, c in enumerate(columns)]
     na_bin = [0 if i in wide else c.na_bin for i, c in enumerate(columns)]
-    ds = _capi.Dataset(byte_bins, num_bins, na_bin, device=device, feature_types=[c.feature_type for c in columns])
+    # (a presorted column starts as a numerical one: set_numerical_column makes it FEATURE_NUMERICAL)
+    types = [_capi.FEATURE_DISCRETIZED_NUMERICAL if _presorted(c) else c.feature_type for c in columns]
+    ds = _capi.Dataset(byte_bins, num_bins, na_bin, device=device, feature_types=types)
     try:
         for i in wide:
             c = columns[i]
-            if c.feature_type == _capi.FEATURE_CATEGORICAL:
+            if _presorted(c):
+                ds.set_numerical_column(i, bins[i], c.mean)
+            elif c.feature_type == _capi.FEATURE_CATEGORICAL:
                 ds.set_wide_categorical_column(i, bins[i], c.num_bins, c.na_bin)
             else:
                 ds.set_wide_column(i, bins[i], c.num_bins, c.na_bin, c.bucket_values, c.mean)

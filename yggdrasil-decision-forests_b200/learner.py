@@ -37,6 +37,7 @@ class GradientBoostedTreesLearner:
                  weights: Optional[str] = None,
                  discretize_numerical_columns: bool = False,
                  max_exact_numerical_values: int = 255,
+                 presort_numerical_columns: bool = False,
                  num_discretized_numerical_bins: int = 255,
                  max_num_scanned_rows_to_compute_statistics: Optional[int] = None,
                  min_vocab_frequency: int = 5,
@@ -101,8 +102,8 @@ class GradientBoostedTreesLearner:
         # is the bucketised split finder, but with one bucket per distinct value it examines exactly the exact splitter's
         # candidate cuts (dataspec.infer_column_lossless; default runs of the reference replayed that way in
         # tests/test_reference_replay.py), so the option is honoured for columns with at most 255 distinct values (byte
-        # buckets), for wider ones up to max_exact_numerical_values (wide columns), and refused — not approximated — for
-        # the others (_build_dataset).
+        # buckets), for wider ones up to max_exact_numerical_values (wide columns), and for the others refused — not
+        # approximated — or, with presort_numerical_columns, split through sorted row lists (_build_dataset).
         self.discretize_numerical_columns = bool(discretize_numerical_columns)
         # The largest numerical column (distinct values) the exact splitter takes.  Columns of up to 255 values use byte
         # buckets; wider ones, up to this limit, become wide columns (uint16 buckets, DESIGN.md §20), whose histogram
@@ -113,6 +114,9 @@ class GradientBoostedTreesLearner:
             raise ValueError(f"max_exact_numerical_values={max_exact_numerical_values} outside [255, 65535] "
                              "(wide columns hold at most 65535 buckets)")
         self.max_exact_numerical_values = int(max_exact_numerical_values)
+        # With the exact splitter, a numerical column with more distinct values than max_exact_numerical_values becomes a
+        # presorted column (float values split through sorted row lists, DESIGN.md §22) instead of being refused.
+        self.presort_numerical_columns = bool(presort_numerical_columns)
         if not 0.0 <= validation_ratio <= 1.0:
             raise ValueError("The validation set ratio should be in [0,1].")
         if early_stopping not in _EARLY_STOPPING:
@@ -191,7 +195,7 @@ class GradientBoostedTreesLearner:
         if self.weights is not None and self.weights in names:
             raise ValueError(f'the weight column "{self.weights}" cannot be a feature')
         n = len(cols[self.label])
-        lossless, categorical = {}, {}
+        lossless, categorical, presorted = {}, {}, {}
         for name in names:   # string columns -> CATEGORICAL (PYDF's semantic inference), checked before the device
             if cols[name].dtype.kind in "OUS":
                 # this learner mirrors PYDF, whose string columns keep most_frequent_value = 0 (dataspec.py)
@@ -210,7 +214,12 @@ class GradientBoostedTreesLearner:
                 if cols[name].dtype.kind in "fiub":
                     limit = self.max_exact_numerical_values
                     lossless[name] = ds_lib.infer_column_lossless(name, cols[name], self.max_rows_stats, max_distinct=limit)
-                    if lossless[name] is None or lossless[name].num_bins > 65535:
+                    if lossless[name] is not None and lossless[name].num_bins <= 65535:
+                        continue
+                    # the path follows the column's cardinality: byte buckets, wide columns up to the limit, presorted above
+                    if self.presort_numerical_columns:
+                        presorted[name] = ds_lib.infer_column_presorted(name, cols[name], self.max_rows_stats)
+                    if presorted.get(name) is None:
                         raise NotImplementedError(
                             f'column "{name}" has more than {limit} distinct values: the exact numerical splitter is only '
                             "reproduced for columns that fit one bucket per value, up to max_exact_numerical_values "
@@ -231,6 +240,10 @@ class GradientBoostedTreesLearner:
                     columns[f] = c
                 elif v.dtype.kind not in "fiub":
                     raise NotImplementedError(f'column "{name}" has unsupported dtype {v.dtype}')
+                elif name in presorted:   # attached after finish(); the byte column is a placeholder
+                    c = presorted[name]
+                    builder.add_bins(f, np.zeros(n, np.uint8), 1, 0, _capi.FEATURE_DISCRETIZED_NUMERICAL)
+                    columns[f] = c
                 elif not self.discretize_numerical_columns:
                     c = lossless[name]
                     if c.wide:   # attached after finish(); the byte column is a placeholder
@@ -258,6 +271,8 @@ class GradientBoostedTreesLearner:
             for f, c in enumerate(columns):
                 if c.feature_type == _capi.FEATURE_CATEGORICAL and c.wide:
                     dataset.set_wide_categorical_column(f, c.encode16(cols[c.name]), c.num_bins, c.na_bin)
+                elif c.feature_type == _capi.FEATURE_NUMERICAL:
+                    dataset.set_numerical_column(f, c.encode(cols[c.name]), c.mean)
             for f, c in enumerate(columns):   # exact numerical splitter: thresholds between the values present in a node
                 if getattr(c, "bucket_values", None) is None:
                     continue

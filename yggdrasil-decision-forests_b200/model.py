@@ -64,10 +64,16 @@ class GradientBoostedTreesModel:
                 idx = rows[active]
                 nd = node[idx]
                 f = t["feature"][nd]
-                b = bins[f, idx].astype(np.int64)
+                raw = bins[f, idx]
+                # presorted numerical splits: value >= threshold_value on the raw float, a missing value -> na_value
+                num = t["condition_type"][nd] == 2
+                b = (np.nan_to_num(raw) if raw.dtype.kind == "f" else raw).astype(np.int64)
                 cat = t["condition_type"][nd] == 1   # (a categorical code is below its column's num_bins <= 32 x width)
                 go_pos = b >= t["threshold_bin"][nd]
                 go_pos[cat] = ((words[nd[cat], b[cat] >> 5] >> (b[cat] & 31).astype(np.uint32)) & 1) != 0
+                if num.any():
+                    v = raw[num]
+                    go_pos[num] = np.where(np.isnan(v), t["na_value"][nd[num]] != 0, v >= t["threshold_value"][nd[num]])
                 node[idx] = np.where(go_pos, t["pos_child"][nd], t["neg_child"][nd])
                 active = t["feature"][node] >= 0
             acc[:, ti % k] += t["leaf_value"][node]

@@ -120,6 +120,10 @@ def encode_data_spec(spec) -> (bytes, int, List[int]):
             cols.append(pb_int(1, 4) + pb_bytes(2, c.name) + pb_int(3, 0) + pb_bytes(6, cat) +
                         pb_int(7, c.num_missing))  # CATEGORICAL
             continue
+        if getattr(c, "feature_type", None) == _capi.FEATURE_NUMERICAL:   # a presorted column: NUMERICAL, Higher splits
+            num = pb_f64(1, c.mean) + pb_f32(2, c.min_value) + pb_f32(3, c.max_value)
+            cols.append(pb_int(1, 1) + pb_bytes(2, c.name) + pb_int(3, 0) + pb_bytes(5, num) + pb_int(7, c.num_missing))
+            continue
         num = pb_f64(1, c.mean)
         if len(c.boundaries):
             num += pb_f32(2, float(c.boundaries[0])) + pb_f32(3, float(c.boundaries[-1]))
@@ -184,7 +188,7 @@ def save_ydf_model(model, path: str):
     if getattr(model, "validation_loss", None) is not None:
         d.has_validation_loss, d.validation_loss = 1, float(model.validation_loss)
         d.early_stopping_triggered = int(bool(getattr(model, "early_stopping_triggered", False)))
-    nvals = np.asarray([c.num_bins for c in model.data_spec.columns], dtype=np.int32)
+    nvals = np.asarray([getattr(c, "num_bins", 0) for c in model.data_spec.columns], dtype=np.int32)
     d.feature_num_values = nvals.ctypes.data_as(C.POINTER(C.c_int32))
     # positive sets of the splits on wide categorical columns
     sets = getattr(model, "category_sets", None) or [{} for _ in model.trees]
