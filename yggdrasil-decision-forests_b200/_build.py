@@ -9,7 +9,7 @@ LIB = os.environ.get("YGG_B200_LIB") or os.path.join(HERE, "libygg_b200.so")
 EXTRA_FLAGS = os.environ.get("YGG_B200_NVCC_FLAGS", "").split()
 SOURCES = ["ygg_engine.cu", "ygg_dataspec.cc", "ygg_model_io.cc", "ygg_comm.cc", "ygg_binning.cu"]
 HEADERS = ["ygg_device.cuh", "ygg_kernels.cuh", "../../include/ygg_b200.h",
-           "../../include/ygg_b200_dataspec.h", "../../include/ygg_b200_model.h", "ygg_hist.cuh", "ygg_wide.cuh", "ygg_presort.cuh",
+           "../../include/ygg_b200_dataspec.h", "../../include/ygg_b200_model.h", "ygg_hist.cuh", "ygg_hist_seg.cuh", "ygg_wide.cuh", "ygg_presort.cuh",
            "../../include/ygg_b200_comm.h", "ygg_internal.h"]
 
 NVCC_FLAGS = [

@@ -44,11 +44,11 @@ FEATURE_DISCRETIZED_NUMERICAL = 0
 FEATURE_CATEGORICAL = 1
 FEATURE_NUMERICAL = 2   # presorted numerical column (Dataset.set_numerical_column)
 
-HIST_ROOT_SUM, HIST_PACKED, HIST_SHARED, HIST2 = 0, 1, 2, 3   # enum ygg_hist_mode
+HIST_ROOT_SUM, HIST_PACKED, HIST_SHARED, HIST2, HIST_SEGMENTED = 0, 1, 2, 3, 4   # enum ygg_hist_mode
 
 
 class HistPlan(C.Structure):
-    """One level's k_hist / k_hist2 launch (ygg_hist_plan)."""
+    """One level's k_hist / k_hist2 / k_hist_seg launch (ygg_hist_plan)."""
     _fields_ = [("mode", C.c_int32), ("group", C.c_int32), ("hist2_tiles", C.c_int32), ("chunk_blocks", C.c_int32),
                 ("slot_window", C.c_int32), ("grid", C.c_int32)]
 

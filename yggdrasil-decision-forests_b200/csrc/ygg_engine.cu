@@ -31,6 +31,7 @@
 #include "ygg_kernels.cuh"
 #include "ygg_wide.cuh"
 #include "ygg_presort.cuh"
+#include "ygg_hist_seg.cuh"
 
 using namespace ygg;
 
@@ -131,6 +132,7 @@ struct HistLaunch {
   int chunk, grid;     // row blocks per work item, CTAs
   int window, passes;  // window > 0: k_hist<., ., MULTI> over `passes` windows of `window` slots
   int FL, T;           // FL > 0: k_hist2 with FL feature lanes and T sub-tiles per tile
+  int SL;              // SL > 0: k_hist_seg with SL feature lanes over S slots (mode kHistPacked, no window)
 };
 
 struct ygg_gbt {
@@ -286,6 +288,15 @@ struct ygg_gbt {
   // launch configuration
   HistLaunch hist_plan[32]{};   // per tree level
   int part_smem_children = 0;
+  // k_hist_seg's node-segmented active rows (ygg_hist_seg.cuh), allocated on first use: seg [n_pad], seg_blk
+  // [kSegMaxSlots][n_blocks], seg_off [kSegMaxSlots * n_blocks + 1], seg_piece [same], seg_meta [4]
+  uint2* d_hseg = nullptr;
+  long long* d_hseg_blk = nullptr;
+  long long* d_hseg_off = nullptr;
+  int32_t* d_hseg_piece = nullptr;
+  int32_t* d_hseg_meta = nullptr;
+  void* d_hseg_temp = nullptr;     // cub's scan scratch
+  size_t hseg_temp_bytes = 0;
   // profiling
   bool profiling = false;
   std::map<std::string, ProfileSlot> profile;
@@ -492,7 +503,8 @@ int chunk_max_count(ygg_gbt* h, int chunk_blocks, uint32_t** d_sub, uint32_t* ou
 }
 
 // Raises the dynamic shared-memory cap of every histogram kernel to its budget, once per device: the seven k_hist
-// instantiations for_hist_kernel returns and the six of k_hist2.  The cap only allows a launch to request that much
+// instantiations for_hist_kernel returns, the six of k_hist2 and the three of k_hist_seg.  The cap only allows a launch
+// to request that much
 // (every launch passes its exact size); it is per kernel and shared by every handle of the process (several handles
 // with different feature shards may coexist), hence always the full budget.
 int raise_hist_smem_caps_once(int device) {
@@ -516,6 +528,14 @@ int raise_hist_smem_caps_once(int device) {
   YGG_RETURN_IF_ERROR(cap2(k_hist2<32, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<32, false>));
   YGG_RETURN_IF_ERROR(cap2(k_hist2<16, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<16, false>));
   YGG_RETURN_IF_ERROR(cap2(k_hist2<8, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<8, false>));
+  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(32))(k_hist_seg<32>));
+  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(16))(k_hist_seg<16>));
+  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(8))(k_hist_seg<8>));
+  // k_hist_seg: the largest shared-memory carveout, the configuration measured in DESIGN.md §5 (the driver's default was
+  // not measured against it)
+  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<16>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<8>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   done[device] = 1;
   return YGG_OK;
 }
@@ -561,6 +581,7 @@ int configure_launches(ygg_gbt* h) {
   const int g_begin = h->hist_f_begin / 4, n_groups = (h->hist_f_end + 3) / 4 - g_begin;
   const char* env_hist2 = std::getenv("YGG_HIST2");
   const bool want_hist2 = env_hist2 != nullptr && std::atoi(env_hist2) != 0;
+  HistLaunch khist_plan[32]{};   // k_hist's plan of each level, the fallback of a k_hist_seg level
   for (int l = 0; l < h->num_levels; l++) {
     HistLaunch& pl = h->hist_plan[l];
     // The root skips the count atomics: its counts are gradient independent and precomputed (a sampled root is not the
@@ -601,6 +622,25 @@ int configure_launches(ygg_gbt* h) {
     const bool packed = pl.mode == kHistPacked || (pl.FL > 0 && l > 0);   // (k_hist2 is not used at a sampled root: its mode is not kHistRootSum)
     const int n_fgroups = pl.FL > 0 ? (n_groups + pl.FL / 4 - 1) / (pl.FL / 4) : (f_count + G - 1) / G;
     pl.chunk = choose_chunk(n_fgroups, pl.grid, packed ? kSubBlocks : 1, pl.FL > 0 ? min_items2 : min_items);
+    pl.SL = 0;
+    khist_plan[l] = pl;
+    // k_hist_seg (one slot per CTA, node-segmented rows of the row-major copy; ygg_hist_seg.cuh) on the packed levels with
+    // at least kSegMinSlots slots: there k_hist's G is small and every level streams the whole matrix for ~30 % of its
+    // rows (DESIGN.md §5).  Its pieces are balanced by a work counter, so the chunk is the largest the packed bound allows
+    // (fewest flushes); confirmed below like k_hist's.
+    const int S_level = level_slot_bound(h, l);
+    if (!hh && pl.mode == kHistPacked && pl.FL == 0 && S_level >= kSegMinSlots) {
+      int SL = 32;
+      while (SL > 8 && SL / 2 >= f_count) SL /= 2;   // few features: fewer idle lanes
+      pl.SL = SL;
+      pl.G = 1;
+      pl.S = S_level;
+      pl.window = 0;
+      pl.passes = 1;
+      pl.grid = h->ds->num_sms * kSegMinBlocks;
+      pl.chunk = std::min(std::max(kSubBlocks, kHistMaxChunkBlocks / kSubBlocks * kSubBlocks),
+                          (n_blocks + kSubBlocks - 1) / kSubBlocks * kSubBlocks);
+    }
   }
   // Packed words (kHistPacked and k_hist2 below the root): the dataset-level bound on the updates a bin can receive
   // inside one work item (ygg_hist.cuh).
@@ -629,6 +669,7 @@ int configure_launches(ygg_gbt* h) {
         chunk = (next < kSubBlocks && chunk > kSubBlocks) ? kSubBlocks : next;
       }
       if (chunk < kSubBlocks) {   // heavy bins (a dominant value / category): the carry-detecting layout, any chunk size
+        if (pl.SL > 0) pl = khist_plan[l];   // k_hist's own geometry of the level (k_hist_seg has only the packed words)
         pl.mode = kHistShared;
         pl.FL = 0;
         pl.chunk = choose_chunk((f_count + pl.G - 1) / pl.G, pl.grid, 1, min_items);
@@ -938,6 +979,93 @@ int launch_hist2(ygg_gbt* h, const Hist2Params& hp, int FL, bool root, int grid)
   return root ? go(k_hist2<8, true>) : go(k_hist2<8, false>);
 }
 
+// The row-major copy of the matrix k_hist_seg gathers from (ygg_hist_seg.cuh), built on first use and kept with the dataset.
+// Published only once it is complete: a failed build leaves the dataset without a copy (the next use retries).
+int ensure_bins_rows(ygg_dataset* ds) {
+  static std::mutex mu;   // handles of one dataset may run in several threads (one per rank)
+  std::lock_guard<std::mutex> lock(mu);
+  if (ds->d_bins_rows != nullptr) return YGG_OK;
+  const int row_bytes = seg_row_bytes(ds->F);
+  uint8_t* rows = nullptr;
+  YGG_RETURN_IF_ERROR(dev_alloc(&rows, static_cast<size_t>(row_bytes) * ds->n_pad));
+  dim3 grid(static_cast<unsigned>((ds->n_pad + 255) / 256), static_cast<unsigned>(row_bytes / 32));
+  k_bins_to_rows<<<grid, 256>>>(ds->d_bins, ds->n_pad, ds->F, row_bytes, rows);
+  int st = check_launch("k_bins_to_rows");
+  if (st == YGG_OK && cudaDeviceSynchronize() != cudaSuccess) st = set_error(YGG_ERR_CUDA, "k_bins_to_rows failed");
+  if (st != YGG_OK) {
+    dev_free(rows);
+    return st;
+  }
+  ds->d_bins_rows = rows;
+  return YGG_OK;
+}
+
+// k_hist_seg's per-level scratch, sized for any level of the handle (<= kSegMaxSlots slots, chunks of >= 1 block).  All
+// or nothing: after a failed allocation (device memory) none of the buffers is kept, and the next use retries.
+void free_seg_buffers(ygg_gbt* h) {
+  dev_free(h->d_hseg); dev_free(h->d_hseg_blk); dev_free(h->d_hseg_off); dev_free(h->d_hseg_piece); dev_free(h->d_hseg_meta);
+  dev_free(h->d_hseg_temp);
+  h->d_hseg = nullptr; h->d_hseg_blk = nullptr; h->d_hseg_off = nullptr; h->d_hseg_piece = nullptr; h->d_hseg_meta = nullptr;
+  h->d_hseg_temp = nullptr;
+  h->hseg_temp_bytes = 0;
+}
+int ensure_seg_buffers(ygg_gbt* h) {
+  if (h->d_hseg_temp != nullptr) return YGG_OK;   // allocated last
+  const size_t ranges = static_cast<size_t>(kSegMaxSlots) * h->n_blocks;
+  auto alloc_all = [&]() -> int {
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_hseg, static_cast<size_t>(h->ds->n_pad)));
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_hseg_blk, ranges));
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_hseg_off, ranges + 1));
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_hseg_piece, ranges + 1));
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_hseg_meta, 4));
+    size_t temp_bytes = 0;
+    YGG_CUDA(cub::DeviceScan::InclusiveSum(nullptr, temp_bytes, h->d_hseg_blk, h->d_hseg_blk, static_cast<int>(ranges)));
+    char* temp = nullptr;
+    YGG_RETURN_IF_ERROR(dev_alloc(&temp, temp_bytes));
+    h->hseg_temp_bytes = temp_bytes;
+    h->d_hseg_temp = temp;
+    return YGG_OK;
+  };
+  const int st = alloc_all();
+  if (st != YGG_OK) free_seg_buffers(h);
+  return st;
+}
+
+// k_hist_seg for level l: the node-segmented rows of the level's active lists (count, scan, ranges, scatter), then the kernel.
+int launch_hist_seg(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* levels, const HistLaunch& pl) {
+  ygg_dataset* ds = h->ds;
+  YGG_RETURN_IF_ERROR(ensure_bins_rows(ds));
+  YGG_RETURN_IF_ERROR(ensure_seg_buffers(h));
+  const int f_count = h->hist_f_end - h->hist_f_begin;
+  const int n_chunks = (h->n_blocks + pl.chunk - 1) / pl.chunk;
+  const int n_fg = (f_count + pl.SL - 1) / pl.SL;
+  const int target_pieces = std::max(1, (kSegItemsPerCta * pl.grid + n_fg - 1) / n_fg);
+  k_seg_count<<<std::min(h->n_blocks, ds->num_sms * 8), 256, 0, h->stream>>>(h->d_act, h->d_act_count, h->n_blocks, pl.S,
+                                                                               levels, l, h->d_hseg_blk);
+  YGG_RETURN_IF_ERROR(check_launch("k_seg_count"));
+  YGG_CUDA(cub::DeviceScan::InclusiveSum(h->d_hseg_temp, h->hseg_temp_bytes, h->d_hseg_blk, h->d_hseg_blk, pl.S * h->n_blocks,
+                                         h->stream));
+  k_seg_ranges<<<1, kSegScanThreads, 0, h->stream>>>(h->d_hseg_blk, pl.S, h->n_blocks, pl.chunk, n_chunks, target_pieces,
+                                                     h->d_hseg_off, h->d_hseg_piece, h->d_hseg_meta);
+  YGG_RETURN_IF_ERROR(check_launch("k_seg_ranges"));
+  k_seg_scatter<<<std::min(h->n_blocks, ds->num_sms * 8), 256, 0, h->stream>>>(h->d_act, h->d_act_count, h->n_blocks, pl.S, levels, l,
+                                                               h->d_hseg_blk, h->d_hseg);
+  YGG_RETURN_IF_ERROR(check_launch("k_seg_scatter"));
+  SegParams sp{};
+  sp.rows = ds->d_bins_rows; sp.row_bytes = static_cast<uint32_t>(seg_row_bytes(ds->F));
+  sp.seg = h->d_hseg; sp.seg_off = h->d_hseg_off; sp.piece_start = h->d_hseg_piece; sp.meta = h->d_hseg_meta;
+  sp.n_ranges = pl.S * n_chunks; sp.n_chunks = n_chunks;
+  sp.f_begin = h->hist_f_begin; sp.f_count = f_count;
+  sp.hist_sum = lb.sum; sp.hist_cnt = lb.cnt;
+  sp.f_chunk = lb.f_chunk; sp.chunk_stride = static_cast<long long>(lb.chunk_u64);
+  const size_t smem = seg_smem_bytes(pl.SL);
+  if (pl.SL == 32) k_hist_seg<32><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
+  else if (pl.SL == 16) k_hist_seg<16><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
+  else k_hist_seg<8><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
+  h->launches_total += 5;
+  return check_launch("k_hist_seg");
+}
+
 // Root count histogram: once per (dataset, shard).
 int ensure_root_counts(ygg_gbt* h) {
   if (h->root_cnt_valid) return YGG_OK;
@@ -970,6 +1098,7 @@ int accumulate_level(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* lev
     YGG_CUDA(cudaMemcpy2DAsync(lb.cnt, lb.chunk_u64 * sizeof(unsigned long long), h->d_root_cnt, row, row, lb.W,
                                cudaMemcpyDeviceToDevice, h->stream));
   }
+  if (pl.SL > 0) return launch_hist_seg(h, l, lb, levels, pl);
   if (pl.FL > 0) {
     YGG_RETURN_IF_ERROR(ensure_bins4(h->ds));
     Hist2Params hp{};
@@ -2119,8 +2248,10 @@ int set_filler_column(ygg_dataset* ds, int32_t feature) {
   std::vector<uint8_t> filler(ds->n);
   for (int64_t r = 0; r < ds->n; r++) filler[r] = static_cast<uint8_t>(r & 0xFF);
   YGG_CUDA(cudaMemcpy(ds->d_bins + static_cast<int64_t>(feature) * ds->n_pad, filler.data(), ds->n, cudaMemcpyHostToDevice));
-  dev_free(ds->d_bins4);   // k_hist2's interleaved copy is rebuilt on first use
+  dev_free(ds->d_bins4);   // k_hist2's interleaved copy and k_hist_seg's row-major copy are rebuilt on first use
   ds->d_bins4 = nullptr;
+  dev_free(ds->d_bins_rows);
+  ds->d_bins_rows = nullptr;
   ds->num_bins[feature] = 1;
   ds->na_bin[feature] = 0;
   return ygg_internal_dataset_finalize(ds);
@@ -2269,11 +2400,16 @@ int ygg_dataset_get_numerical_column(const ygg_dataset* ds, int32_t feature, flo
 
 int ygg_dataset_destroy(ygg_dataset* ds) {
   if (!ds) return YGG_OK;
+  if (ds->handles > 0) {   // handles still use it: the last ygg_gbt_destroy releases it
+    ds->destroy_pending = true;
+    return YGG_OK;
+  }
   cudaSetDevice(ds->device);
   dev_free(ds->d_wide); dev_free(ds->d_wide_of); dev_free(ds->d_wide_off); dev_free(ds->d_wide_values);
   dev_free(ds->d_num); dev_free(ds->d_num_of);
   dev_free(ds->d_bins);
   dev_free(ds->d_bins4);
+  dev_free(ds->d_bins_rows);
   dev_free(ds->d_num_bins);
   dev_free(ds->d_na_bin);
   dev_free(ds->d_feature_type);
@@ -2451,11 +2587,11 @@ static int init_handle(ygg_gbt* h) {
 int ygg_gbt_destroy(ygg_gbt* h) {
   if (!h) return YGG_OK;
   cudaSetDevice(h->ds->device);
-  if (h->counted) h->ds->handles--;
   if (h->stream) cudaStreamSynchronize(h->stream);
   collect_profile(h);
   dev_free(h->d_label_u8); dev_free(h->d_label_f32); dev_free(h->d_pred); dev_free(h->d_g); dev_free(h->d_h);
   dev_free(h->d_q24); dev_free(h->d_hq24); dev_free(h->d_act); dev_free(h->d_act_h);
+  free_seg_buffers(h);
   dev_free(h->d_act_count); dev_free(h->d_act_sub); dev_free(h->d_root_cnt); dev_free(h->d_node_of_row); dev_free(h->d_st); dev_free(h->d_levels);
   for (int i = 0; i < 2; i++) {
     dev_free(h->d_fam[i]); dev_free(h->d_slot_node[i]); dev_free(h->d_hist_sum[i]); dev_free(h->d_hist_cnt[i]);
@@ -2477,7 +2613,10 @@ int ygg_gbt_destroy(ygg_gbt* h) {
   cudaFree(h->d_goss_temp);
   cudaFree(h->d_level_buf);
   if (h->stream) cudaStreamDestroy(h->stream);
+  ygg_dataset* ds = h->ds;
+  const bool counted = h->counted;
   delete h;
+  if (counted && --ds->handles == 0 && ds->destroy_pending) return ygg_dataset_destroy(ds);
   return YGG_OK;
 }
 
@@ -3282,6 +3421,8 @@ int ygg_debug_hist_plan(const ygg_gbt* h, int32_t level, ygg_hist_plan* out) {
   ygg_hist_plan p{};
   if (pl.FL > 0) {
     p.mode = YGG_HIST_HIST2; p.group = pl.FL; p.hist2_tiles = pl.T;
+  } else if (pl.SL > 0) {
+    p.mode = YGG_HIST_SEGMENTED; p.group = pl.SL;
   } else {
     p.mode = pl.mode == kHistRootSum ? YGG_HIST_ROOT_SUM : pl.mode == kHistPacked ? YGG_HIST_PACKED : YGG_HIST_SHARED;
     p.group = pl.G;
@@ -3323,7 +3464,7 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
       return set_error(YGG_ERR_INVALID_ARGUMENT, "the plan of level %d holds %d slots, %d requested", level, level_slot_bound(h, level), n_slots);
   } else {
     const ygg_hist_plan& p = *plan;
-    if (p.mode < YGG_HIST_ROOT_SUM || p.mode > YGG_HIST_HIST2) return set_error(YGG_ERR_INVALID_ARGUMENT, "unknown mode %d", p.mode);
+    if (p.mode < YGG_HIST_ROOT_SUM || p.mode > YGG_HIST_SEGMENTED) return set_error(YGG_ERR_INVALID_ARGUMENT, "unknown mode %d", p.mode);
     if (p.chunk_blocks < 1 || p.chunk_blocks > kHistMaxChunkBlocks)
       return set_error(YGG_ERR_INVALID_ARGUMENT, "chunk_blocks=%d outside [1, %d]", p.chunk_blocks, kHistMaxChunkBlocks);
     if (p.grid < 1 || p.grid > 65535) return set_error(YGG_ERR_INVALID_ARGUMENT, "grid=%d outside [1, 65535]", p.grid);
@@ -3338,6 +3479,13 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
         return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist2 needs %zu bytes of shared memory (budget 216 KB)", hist2_smem_bytes(p.group, n_slots, p.hist2_tiles, level == 0));
       pl.FL = p.group; pl.T = p.hist2_tiles; pl.S = n_slots; pl.G = 1; pl.passes = 1;
       pl.mode = level == 0 ? kHistRootSum : kHistPacked;
+    } else if (p.mode == YGG_HIST_SEGMENTED) {
+      if (level == 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist_seg runs below the root only");
+      if (hh) return set_error(YGG_ERR_INVALID_ARGUMENT, "a second histogram plane is accumulated by the shared layout only");
+      if (p.group != 8 && p.group != 16 && p.group != 32) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist_seg: %d feature lanes (8, 16 or 32)", p.group);
+      if (p.slot_window != 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist_seg has no multi-pass form");
+      pl.SL = p.group; pl.S = n_slots; pl.G = 1; pl.passes = 1;
+      pl.mode = kHistPacked;
     } else {
       if (p.group < 1 || p.group > 8) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist: group=%d outside [1, 8]", p.group);
       pl.mode = p.mode == YGG_HIST_ROOT_SUM ? kHistRootSum : p.mode == YGG_HIST_PACKED ? kHistPacked : kHistShared;
@@ -3355,7 +3503,7 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
                          pl.G, pl.S, hist_smem_bytes(pl.G, pl.S, hh, pl.mode), budget);
     }
   }
-  if (hh && (pl.FL > 0 || pl.mode != kHistShared))
+  if (hh && (pl.FL > 0 || pl.SL > 0 || pl.mode != kHistShared))
     return set_error(YGG_ERR_INVALID_ARGUMENT, "a second histogram plane is accumulated by the shared layout only");
   if (pl.mode == kHistRootSum && (level != 0 || sampling(h) || !all_slot0 || n_slots != 1))
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the root layouts need level 0, no row sampling and every row in slot 0");

@@ -14,6 +14,7 @@ struct ygg_dataset {
   int F = 0;
   uint8_t* d_bins = nullptr;
   uint32_t* d_bins4 = nullptr;   // interleaved copy [ceil(F/4)][n_pad] for k_hist2 (built on first use, ygg_hist2.cuh)
+  uint8_t* d_bins_rows = nullptr;   // row-major copy [n_pad][F rounded up to 32] for k_hist_seg (built on first use, ygg_hist_seg.cuh)
   int32_t* d_num_bins = nullptr;
   int32_t* d_na_bin = nullptr;
   int32_t* d_feature_type = nullptr;
@@ -50,6 +51,7 @@ struct ygg_dataset {
   std::vector<float> num_na_replacement;
   int n_num() const { return static_cast<int>(num_feature.size()); }
   int handles = 0;                     // live ygg_gbt handles on this dataset (wide columns are set before the first)
+  bool destroy_pending = false;        // ygg_dataset_destroy ran while handles were live: the last handle's destroy frees it
 };
 
 __attribute__((visibility("hidden"))) int ygg_internal_dataset_alloc(ygg_dataset** out, int64_t n_rows,
