@@ -405,7 +405,8 @@ enum ygg_hist_mode {
 };
 typedef struct ygg_hist_plan {  /* one level's k_hist / k_hist2 / k_hist_seg launch */
   int32_t mode;            /* enum ygg_hist_mode */
-  int32_t group;           /* features per work item G (k_hist, 1..8), or feature lanes FL (k_hist2, k_hist_seg: 8, 16, 32) */
+  int32_t group;           /* features per work item G (k_hist, 1..8), or feature lanes FL (k_hist2, k_hist_seg: 8, 16, 32;
+                              k_hist_seg at 32 lanes over more than 32 features takes two adjacent features per lane) */
   int32_t hist2_tiles;     /* sub-tiles of 1024 rows per tile T (k_hist2 only: 1, 2) */
   int32_t chunk_blocks;    /* 8192-row blocks per work item, 1..127 */
   int32_t slot_window;     /* 0: one pass over every slot; else slots per pass (multi-pass k_hist + one dummy slot) */

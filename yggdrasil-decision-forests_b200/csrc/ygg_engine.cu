@@ -503,7 +503,7 @@ int chunk_max_count(ygg_gbt* h, int chunk_blocks, uint32_t** d_sub, uint32_t* ou
 }
 
 // Raises the dynamic shared-memory cap of every histogram kernel to its budget, once per device: the seven k_hist
-// instantiations for_hist_kernel returns, the six of k_hist2 and the three of k_hist_seg.  The cap only allows a launch
+// instantiations for_hist_kernel returns, the six of k_hist2 and the four of k_hist_seg.  The cap only allows a launch
 // to request that much
 // (every launch passes its exact size); it is per kernel and shared by every handle of the process (several handles
 // with different feature shards may coexist), hence always the full budget.
@@ -528,14 +528,16 @@ int raise_hist_smem_caps_once(int device) {
   YGG_RETURN_IF_ERROR(cap2(k_hist2<32, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<32, false>));
   YGG_RETURN_IF_ERROR(cap2(k_hist2<16, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<16, false>));
   YGG_RETURN_IF_ERROR(cap2(k_hist2<8, true>)); YGG_RETURN_IF_ERROR(cap2(k_hist2<8, false>));
-  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(32))(k_hist_seg<32>));
-  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(16))(k_hist_seg<16>));
-  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(8))(k_hist_seg<8>));
+  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(64))(k_hist_seg<32, 2>));
+  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(32))(k_hist_seg<32, 1>));
+  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(16))(k_hist_seg<16, 1>));
+  YGG_RETURN_IF_ERROR(set_cap(seg_smem_bytes(8))(k_hist_seg<8, 1>));
   // k_hist_seg: the largest shared-memory carveout, the configuration measured in DESIGN.md §5 (the driver's default was
   // not measured against it)
-  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<16>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<8>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<32, 2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<32, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<16, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<8, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   done[device] = 1;
   return YGG_OK;
 }
@@ -1038,7 +1040,8 @@ int launch_hist_seg(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* leve
   YGG_RETURN_IF_ERROR(ensure_seg_buffers(h));
   const int f_count = h->hist_f_end - h->hist_f_begin;
   const int n_chunks = (h->n_blocks + pl.chunk - 1) / pl.chunk;
-  const int n_fg = (f_count + pl.SL - 1) / pl.SL;
+  const int fpl = seg_lane_features(pl.SL, f_count);
+  const int n_fg = seg_feature_groups(pl.SL, fpl, h->hist_f_begin, f_count);
   const int target_pieces = std::max(1, (kSegItemsPerCta * pl.grid + n_fg - 1) / n_fg);
   k_seg_count<<<std::min(h->n_blocks, ds->num_sms * 8), 256, 0, h->stream>>>(h->d_act, h->d_act_count, h->n_blocks, pl.S,
                                                                                levels, l, h->d_hseg_blk);
@@ -1058,10 +1061,11 @@ int launch_hist_seg(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* leve
   sp.f_begin = h->hist_f_begin; sp.f_count = f_count;
   sp.hist_sum = lb.sum; sp.hist_cnt = lb.cnt;
   sp.f_chunk = lb.f_chunk; sp.chunk_stride = static_cast<long long>(lb.chunk_u64);
-  const size_t smem = seg_smem_bytes(pl.SL);
-  if (pl.SL == 32) k_hist_seg<32><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
-  else if (pl.SL == 16) k_hist_seg<16><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
-  else k_hist_seg<8><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
+  const size_t smem = seg_smem_bytes(pl.SL * fpl);
+  if (fpl == 2) k_hist_seg<32, 2><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
+  else if (pl.SL == 32) k_hist_seg<32, 1><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
+  else if (pl.SL == 16) k_hist_seg<16, 1><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
+  else k_hist_seg<8, 1><<<pl.grid, kSegThreads, smem, h->stream>>>(sp);
   h->launches_total += 5;
   return check_launch("k_hist_seg");
 }

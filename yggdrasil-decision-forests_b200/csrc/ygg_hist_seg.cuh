@@ -9,13 +9,17 @@
 //                  (row block, row) order (k_seg_count, cub's inclusive scan, k_seg_ranges, k_seg_scatter, from the
 //                  per-block lists d_act);
 //   seg_off[r]     start of range r = slot * n_chunks + chunk (chunk = `chunk_blocks` consecutive row blocks), [R + 1].
-// Work item = (piece of one range of at most P entries) x (group of FL features).  A CTA holds ONE slot of FL features
-// in shared memory, [bin][plane][feature] packed words as kHistPacked (ygg_hist.cuh): lane = feature, so the two
-// non-returning atomics of a row hit 32 different banks.  A warp gathers, per row, one byte per lane from the row's
-// sector.  A piece is a subset of one (slot, chunk) range, and a chunk's rows give every bin at most as many updates as
-// the chunk_max_count bound checks: the packed words stay exact.  Pieces are taken from a work counter (slot sizes
+// Work item = (piece of one range of at most P entries) x (group of FL x FPL features: FPL features per lane, 1 or 2).
+// A CTA holds ONE slot of the group in shared memory, [bin][plane][half][lane] packed words as kHistPacked
+// (ygg_hist.cuh), so that at 32 lanes every atomic of a warp instruction hits bank = lane.  A warp gathers, per row, FPL
+// adjacent bytes per lane: FPL = 1 is one 32-byte sector per row and group, FPL = 2 (FL = 32, shards of more than 32
+// features) two sectors in ONE load request, the requests per row halved.  A paired group starts at an even byte of the
+// row (the shard's first feature rounded down) so that every 2-byte load is aligned; its columns outside the shard are
+// accumulated and dropped.
+// A piece is a subset of one (slot, chunk) range, and a chunk's rows give every bin at most as many updates as the
+// chunk_max_count bound checks: the packed words stay exact.  Pieces are taken from a work counter (slot sizes
 // differ a lot); the feature groups of a piece are consecutive items, so their CTAs read the same rows at about the same
-// time and a row's other sectors come from L2 (ldg_u8_row).
+// time and a row's other sectors come from L2 (ldg_row).
 #pragma once
 #include <cstdint>
 #include <type_traits>
@@ -31,13 +35,21 @@ constexpr int kSegThreads = 1024;
 constexpr int kSegMinBlocks = 1;       // CTAs per SM (<= 64 registers: 32 gathers in flight per lane)
 constexpr int kSegMinSlots = 4;        // level slot bound from which the planner takes k_hist_seg (DESIGN.md §5)
 constexpr int kSegItemsPerCta = 4;     // target work items per CTA: sets the piece size P
-constexpr int kSegMinPiece = 4096;     // smallest P: the flush of FL x 256 bins stays small against the piece
+constexpr int kSegMinPiece = 4096;     // smallest P: the flush of FL x FPL x 256 bins stays small against the piece
 constexpr int kSegMaxSlots = 256;      // slots the pass handles (the entries carry 8-bit slots)
 constexpr int kSegScanThreads = 512;
 
-__host__ __device__ inline size_t seg_smem_bytes(int FL) { return static_cast<size_t>(kMaxBins) * 2 * FL * 4; }
+// Features per lane of a launch with FL lanes over a shard of f_count features: two at 32 lanes above 32 features.
+inline int seg_lane_features(int FL, int f_count) { return FL == 32 && f_count > 32 ? 2 : 1; }
+// Shared memory of a work item of FI = FL x FPL features.
+__host__ __device__ inline size_t seg_smem_bytes(int FI) { return static_cast<size_t>(kMaxBins) * 2 * FI * 4; }
+// Feature groups of a shard: FPL = 2 starts its groups at the even byte at or below the shard's first feature.
+__host__ __device__ inline int seg_feature_groups(int FL, int FPL, int f_begin, int f_count) {
+  const int off = FPL == 2 ? (f_begin & 1) : 0;
+  return (f_count + off + FL * FPL - 1) / (FL * FPL);
+}
 // Bytes per row of the row-major copy: the power of two >= F from 32 to 256 (a row is one aligned region of at most
-// 256 bytes: ldg_u8_row), above 256 features a multiple of 256.
+// 256 bytes: ldg_row), above 256 features a multiple of 256.
 inline int seg_row_bytes(int F) {
   int b = 32;
   while (b < F && b < 256) b *= 2;
@@ -183,12 +195,14 @@ __global__ void __launch_bounds__(256) k_seg_scatter(const uint2* act, const int
   }
 }
 
-// One byte of a row, with a hint to fetch the row's whole aligned 256-byte region into L2: the other feature groups of
-// the row are read by the CTAs of the piece's other items at about the same time, so a row costs one 256-byte DRAM
-// access instead of one 32-byte sector access per feature group.
-__device__ __forceinline__ uint32_t ldg_u8_row(const uint8_t* p) {
+// One byte (FPL = 1) or two aligned bytes (FPL = 2, the first in bits 0-7) of a row, with a hint to fetch the row's whole
+// aligned 256-byte region into L2: the other feature groups of the row are read by the CTAs of the piece's other items at
+// about the same time, so a row costs one 256-byte DRAM access instead of one sector access per feature group.
+template <int FPL>
+__device__ __forceinline__ uint32_t ldg_row(const uint8_t* p) {
   uint32_t v;
-  asm("ld.global.nc.L2::256B.u8 %0, [%1];" : "=r"(v) : "l"(p));
+  if constexpr (FPL == 2) asm("ld.global.nc.L2::256B.u16 %0, [%1];" : "=r"(v) : "l"(p));
+  else asm("ld.global.nc.L2::256B.u8 %0, [%1];" : "=r"(v) : "l"(p));
   return v;
 }
 
@@ -207,21 +221,26 @@ struct SegParams {
   long long chunk_stride;
 };
 
-template <int FL>
+template <int FL, int FPL>
 __global__ void __launch_bounds__(kSegThreads, kSegMinBlocks) k_hist_seg(SegParams p) {
   static_assert(FL == 8 || FL == 16 || FL == 32, "feature lanes");
+  static_assert(FPL == 1 || (FPL == 2 && FL == 32), "two features per lane at 32 lanes only");
+  constexpr int FI = FL * FPL;             // features per work item
   constexpr int R = 32 / FL;               // rows per warp step (FL < 32: few features)
   constexpr int kSteps = 32 / R;           // rows per lane per warp iteration of 32 entries
   constexpr int kInFlight = FL == 32 ? 32 : 8;   // gathers issued before their atomics (within 64 registers)
   constexpr int kWarps = kSegThreads / 32;
-  constexpr int kWords = kMaxBins * 2 * FL;
-  extern __shared__ __align__(16) uint32_t s_bins[];   // [bin][plane][feature]
+  constexpr int kWords = kMaxBins * 2 * FI;
+  constexpr uint32_t kBinBytes = 2u * FI * 4u, kPlaneBytes = FI * 4u, kHalfBytes = FL * 4u;
+  extern __shared__ __align__(16) uint32_t s_bins[];   // word ((bin*2 + plane)*FPL + half)*FL + lane
   __shared__ int s_item;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int fl = lane % FL, sub = lane / FL;
   uint32_t s_base = static_cast<uint32_t>(__cvta_generic_to_shared(s_bins));
   asm volatile("mov.u32 %0, %0;" : "+r"(s_base));   // (see k_hist)
-  const int n_fg = (p.f_count + FL - 1) / FL;
+  // FPL = 2: the groups start at the even byte f_begin - off of the row, column 0 of the first group is feature -off
+  const int off = FPL == 2 ? (p.f_begin & 1) : 0;
+  const int n_fg = seg_feature_groups(FL, FPL, p.f_begin, p.f_count);
   const int P = p.meta[0];
   const int n_items = p.meta[1] * n_fg;
   for (int i = tid; i < kWords; i += kSegThreads) s_bins[i] = 0u;
@@ -241,13 +260,15 @@ __global__ void __launch_bounds__(kSegThreads, kSegMinBlocks) k_hist_seg(SegPara
     const long long beg = __ldg(p.seg_off + lo) + static_cast<long long>(piece - __ldg(p.piece_start + lo)) * P;
     const int len = static_cast<int>(min(static_cast<long long>(P), __ldg(p.seg_off + lo + 1) - beg));
     const int slot = lo / p.n_chunks;
-    const int f0 = fg * FL, gcount = min(FL, p.f_count - f0);
-    const uint8_t* col = p.rows + p.f_begin + f0 + min(fl, gcount - 1);   // lanes past the group re-read its last feature
+    const int f0 = fg * FI - off;                     // shard feature of the group's column 0
+    const int last = min(FI, p.f_count - f0) - 1;     // the group's last column inside the shard
+    // lanes past it re-read its last feature (pair): no load leaves the row (a pair ending at an odd byte < row_bytes)
+    const uint8_t* col = p.rows + p.f_begin + f0 + min(fl * FPL, last & ~(FPL - 1));
     const uint2* sp = p.seg + beg;
 
     // A warp takes 32 entries at a time, one per lane (coalesced, loaded one iteration ahead), and issues the gathers of
     // their rows before their atomics (32 in flight per lane at FL = 32).  x = q | 1 << 31 for a row of the piece, 0
-    // past its end (row 0, adding nothing): w0 += coarse << 13 | valid, w1 += q.
+    // past its end (row 0, adding nothing): w0 += coarse << 13 | valid, w1 += q, in the word of each gathered byte.
     int e = warp * 32;
     uint2 cur = e + lane < len ? __ldg(sp + e + lane) : make_uint2(0u, 0u);
     for (; e < len; e += kWarps * 32) {
@@ -260,32 +281,42 @@ __global__ void __launch_bounds__(kSegThreads, kSegMinBlocks) k_hist_seg(SegPara
 #pragma unroll
         for (int j = 0; j < kInFlight; j++) {
           const uint32_t row = __shfl_sync(0xFFFFFFFFu, cur.y, (j0 + j) * R + sub);
-          b[j] = ldg_u8_row(col + static_cast<size_t>(row) * p.row_bytes);
+          b[j] = ldg_row<FPL>(col + static_cast<size_t>(row) * p.row_bytes);
         }
 #pragma unroll
         for (int j = 0; j < kInFlight; j++) {
           const uint32_t x = __shfl_sync(0xFFFFFFFFu, xq, (j0 + j) * R + sub);
-          const uint32_t a = a_lane + b[j] * (2u * FL * 4u);
-          smem_red(a, (((x >> kPackedCoarseShift) & 0x3Fu) << kPackedCntBits) | (x >> 31));
-          smem_red(a + FL * 4u, x & kQMax);
+          const uint32_t inc = (((x >> kPackedCoarseShift) & 0x3Fu) << kPackedCntBits) | (x >> 31), q = x & kQMax;
+          const uint32_t a = a_lane + (FPL == 2 ? b[j] & 0xFFu : b[j]) * kBinBytes;
+          smem_red(a, inc);
+          smem_red(a + kPlaneBytes, q);
+          if constexpr (FPL == 2) {
+            const uint32_t a1 = a_lane + kHalfBytes + (b[j] >> 8) * kBinBytes;
+            smem_red(a1, inc);
+            smem_red(a1 + kPlaneBytes, q);
+          }
         }
       }
       cur = nxt;
     }
     __syncthreads();
 
-    // flush the non-empty bins of the group's features and zero every touched word for the next item
-    for (int i = tid; i < kMaxBins * FL; i += kSegThreads) {
-      const int bin = i / FL, fi = i - bin * FL;
-      uint32_t* w = s_bins + bin * 2 * FL + fi;
+    // flush the non-empty bins of the group's features and zero every touched word for the next item.  A column of the
+    // shard receives <= 8191 updates, so its count is 0 only when both its words are; the others (re-read features,
+    // FPL = 2: the shard's neighbours and the row's zero padding) may receive any number and are always cleared.
+    for (int i = tid; i < kMaxBins * FI; i += kSegThreads) {
+      const int bin = i / FI, k = i - bin * FI;        // k = half * FL + lane
+      const int f = f0 + (k % FL) * FPL + k / FL;      // its shard feature
+      const bool in = f >= 0 && f < p.f_count;
+      uint32_t* w = s_bins + bin * 2 * FI + k;
       const uint32_t c = w[0];
-      if (c == 0u) continue;
-      const uint32_t lo32 = w[FL];
+      if (c == 0u && in) continue;
+      const uint32_t lo32 = w[FI];
       w[0] = 0u;
-      w[FL] = 0u;
-      if (fi >= gcount) continue;
+      w[FI] = 0u;
+      if (!in) continue;
       size_t oc;
-      const size_t o = slot_hist_offset(slot, f0 + fi, bin, p.f_chunk, p.chunk_stride, &oc);
+      const size_t o = slot_hist_offset(slot, f, bin, p.f_chunk, p.chunk_stride, &oc);
       const unsigned long long base = static_cast<unsigned long long>(c >> kPackedCntBits) << kPackedCoarseShift;
       atomicAdd(&p.hist_sum[o], base + static_cast<uint32_t>(lo32 - static_cast<uint32_t>(base)));
       atomicAdd(&p.hist_cnt[oc], c & kPackedMaxUpdates);
