@@ -626,12 +626,13 @@ int configure_launches(ygg_gbt* h) {
     pl.chunk = choose_chunk(n_fgroups, pl.grid, packed ? kSubBlocks : 1, pl.FL > 0 ? min_items2 : min_items);
     pl.SL = 0;
     khist_plan[l] = pl;
-    // k_hist_seg (one slot per CTA, node-segmented rows of the row-major copy; ygg_hist_seg.cuh) on the packed levels with
-    // at least kSegMinSlots slots: there k_hist's G is small and every level streams the whole matrix for ~30 % of its
-    // rows (DESIGN.md §5).  Its pieces are balanced by a work counter, so the chunk is the largest the packed bound allows
-    // (fewest flushes); confirmed below like k_hist's.
+    // k_hist_seg (one slot per CTA, node-segmented rows of the row-major copy; ygg_hist_seg.cuh) on the packed levels below
+    // the root with at least kSegMinSlots slots, and on levels 1-2 too for wide, large shards (seg_min_slots): below the
+    // root k_hist streams the whole matrix for ~30-40 % of its rows, and from 4 slots its G is small (DESIGN.md §5).
+    // Its pieces are balanced by a work counter, so the chunk is the largest the packed bound allows (fewest flushes);
+    // confirmed below like k_hist's.
     const int S_level = level_slot_bound(h, l);
-    if (!hh && pl.mode == kHistPacked && pl.FL == 0 && S_level >= kSegMinSlots) {
+    if (!hh && l > 0 && pl.mode == kHistPacked && pl.FL == 0 && S_level >= seg_min_slots(f_count, h->ds->n)) {
       int SL = 32;
       while (SL > 8 && SL / 2 >= f_count) SL /= 2;   // few features: fewer idle lanes
       pl.SL = SL;

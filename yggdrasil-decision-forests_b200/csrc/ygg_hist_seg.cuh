@@ -1,4 +1,5 @@
-// ygg_hist_seg.cuh — k_hist_seg: the level histograms of the deep tree levels, one node's rows per work item.
+// ygg_hist_seg.cuh — k_hist_seg: the level histograms of the deep tree levels (and of levels 1-2 on wide, large shards),
+// one node's rows per work item.
 //
 // k_hist streams the whole column-major matrix at every level and keeps all S slots of a level in one CTA's shared
 // memory; below level 2 a level accumulates ~30 % of the rows, and S pushes its feature group G down to 2-5.  Here:
@@ -34,6 +35,12 @@ namespace ygg {
 constexpr int kSegThreads = 1024;
 constexpr int kSegMinBlocks = 1;       // CTAs per SM (<= 64 registers: 32 gathers in flight per lane)
 constexpr int kSegMinSlots = 4;        // level slot bound from which the planner takes k_hist_seg (DESIGN.md §5)
+// Levels 1 and 2 (one or two slots) take k_hist_seg on shards of at least this many features and rows x features
+// (measured on C3-shaped data, DESIGN.md §5): per added row it costs as much as k_hist at 100 features and less from 128
+// on, and the whole-matrix stream it saves pays for its grouping pass from ~0.8e9 elements on (200 features: 4M rows
+// break even).
+constexpr int kSegShallowMinFeatures = 128;
+constexpr long long kSegShallowMinElements = 1000000000LL;
 constexpr int kSegItemsPerCta = 4;     // target work items per CTA: sets the piece size P
 constexpr int kSegMinPiece = 4096;     // smallest P: the flush of FL x FPL x 256 bins stays small against the piece
 constexpr int kSegMaxSlots = 256;      // slots the pass handles (the entries carry 8-bit slots)
@@ -41,6 +48,11 @@ constexpr int kSegScanThreads = 512;
 
 // Features per lane of a launch with FL lanes over a shard of f_count features: two at 32 lanes above 32 features.
 inline int seg_lane_features(int FL, int f_count) { return FL == 32 && f_count > 32 ? 2 : 1; }
+// Level slot bound from which the planner takes k_hist_seg for a shard of f_count features over `rows` rows: every
+// level below the root on wide, large shards (paired form), kSegMinSlots otherwise.
+inline int seg_min_slots(int f_count, long long rows) {
+  return f_count >= kSegShallowMinFeatures && rows * f_count >= kSegShallowMinElements ? 1 : kSegMinSlots;
+}
 // Shared memory of a work item of FI = FL x FPL features.
 __host__ __device__ inline size_t seg_smem_bytes(int FI) { return static_cast<size_t>(kMaxBins) * 2 * FI * 4; }
 // Feature groups of a shard: FPL = 2 starts its groups at the even byte at or below the shard's first feature.
