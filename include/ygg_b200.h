@@ -436,6 +436,35 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
  * follow each other in the order they were set. */
 int ygg_debug_wide_histogram(ygg_gbt* h, int32_t n_slots, uint64_t* out_sum, uint32_t* out_cnt, uint64_t* out_second);
 
+/* Split-candidate capture of the level loop.  enabled != 0: every tree the handle grows afterwards copies, at each level,
+ * the complete candidate table left by the scan phase (every node of the level x every feature the handle scans, with the
+ * wide and presorted columns' float thresholds and wide categorical positive sets) into buffers allocated here, before the
+ * selection; the copies are asynchronous.  enabled == 0 frees them: the level loop is then exactly as without capture. */
+int ygg_debug_capture_candidates(ygg_gbt* h, int32_t enabled);
+typedef struct ygg_level_node {
+  int32_t node;            /* pre-order index in the emitted tree */
+  int32_t candidate;       /* 1: the node was scanned (it may be split) */
+  int32_t derived;         /* 1: its histogram was parent - sibling; 0: accumulated from its rows */
+  int32_t reserved;
+  int64_t num_examples;
+} ygg_level_node;
+typedef struct ygg_candidate {
+  int32_t found;
+  float score;
+  int32_t threshold_bin;   /* thr_bin_of: bin >= threshold_bin is positive (1 for a presorted column) */
+  int32_t lo, hi;          /* the exact threshold rule's buckets around the cut (byte columns with bucket values), else -1 */
+  int32_t num_pos_examples;
+  float threshold_value;   /* float threshold of an exact-rule, wide numerical or presorted candidate, else NaN */
+  uint32_t cat_mask[8];    /* positive categories of a byte categorical candidate */
+} ygg_candidate;
+/* The capture of tree level `level` of the last tree grown with capture enabled (a ygg_tree_train_on_gradients tree,
+ * level-wise growth, candidate_shuffle = 0).  nodes[capacity], cands[capacity][features scanned by this handle], sets
+ * (or NULL) [capacity][wide features][set_words] of the wide categorical candidates; *n_nodes = the level's nodes;
+ * scales = {P, the hessian plane's power of two, the weight plane's power of two}.  INVALID_ARGUMENT on a null handle or
+ * output, a level outside the captured tree, a capacity below the level's nodes or no capture. */
+int ygg_debug_level_candidates(ygg_gbt* h, int32_t level, int32_t capacity, ygg_level_node* nodes, ygg_candidate* cands,
+                               uint32_t* sets, int32_t set_words, int32_t* n_nodes, float* scales);
+
 /* SplitExamplesInPlace seam (learner/decision_tree/training.cc:5243-5305 ->
  * model/decision_tree/decision_tree.cc:957-1012): stable two-way partition of a row-id list by
  * `bin(feature,row) >= threshold_bin`; positives then negatives, both ascending-stable.  YGG_ERR_UNIMPLEMENTED on a

@@ -1,18 +1,16 @@
 """Numpy reference of the exact numerical splitter on one node (DESIGN.md §22), shared by the presorted column tests.
 
 The node's rows are grouped by distinct value (missing values already replaced by the column mean), every boundary
-between two consecutive distinct values is scored with the byte and wide scans' formulas (tests/wide_cat_ref.scores
+between two consecutive distinct values is scored with the byte and wide scans' formulas (tests/scan_ref.prescreen
 over the values in ascending order), and the first maximum wins.  The threshold is MidThreshold of the two values
 around the cut (learner/decision_tree/utils.h:103-109) in float32."""
 import numpy as np
 
+from tests import scan_ref as S
 from tests import wide_cat_ref as W
 
 
-def mid_threshold(a, b) -> np.float32:
-    a, b = np.float32(a), np.float32(b)
-    t = np.float32(a + np.float32((b - a) / np.float32(2)))
-    return b if t <= a else t
+mid_threshold = S.mid_threshold
 
 
 def best_split(values, g_units, h_units=None, use_hessian=False, min_obs=1, w_units=None, subtract_parent=False, l2=0.0):
@@ -26,7 +24,7 @@ def best_split(values, g_units, h_units=None, use_hessian=False, min_obs=1, w_un
     s = np.bincount(inv, weights=g_units, minlength=len(distinct))
     h = np.bincount(inv, weights=h_units, minlength=len(distinct)) if use_hessian else cnt
     w = None if w_units is None else np.bincount(inv, weights=w_units, minlength=len(distinct))
-    sc, npos = W.scores(cnt, s, h, np.arange(len(distinct)), use_hessian, min_obs, l2, w, subtract_parent)
+    sc, npos = S.prescreen(cnt, s, h, np.arange(len(distinct)), use_hessian, min_obs, l2, w, subtract_parent)
     if sc.max() < 0:
         return None
     b = int(np.argmax(sc))   # the first maximum in ascending value order

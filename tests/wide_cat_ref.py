@@ -6,7 +6,7 @@ hessian priority with l2_categorical), categories sorted ascending by (key, inde
 positions scored, the first maximum kept; the categories after it form the positive set."""
 import numpy as np
 
-MIN_HESSIAN = 0.001   # kMinHessianForNewtonStep
+from tests.scan_ref import MIN_HESSIAN, prescreen as scores  # noqa: F401 (the scores are the scan reference's)
 
 
 def keys(cnt, s, h, use_hessian, l2_categorical=1.0, weight=None):
@@ -18,36 +18,6 @@ def keys(cnt, s, h, use_hessian, l2_categorical=1.0, weight=None):
     with np.errstate(invalid="ignore", divide="ignore"):
         k = (s / (h + l2_categorical)).astype(np.float32).astype(np.float64)
     return np.where(h > 0, k, 0.0)
-
-
-def scores(cnt, s, h, order, use_hessian, min_obs=1, l2_categorical=1.0, weight=None, subtract_parent=False):
-    """Scores of the boundaries after sorted positions 0..B-2 (-1 where not valid) and the positive counts.  `weight`:
-    per-category weight sums, which take the place of the counts in the variance score (the counts keep deciding
-    min_obs).  subtract_parent: the hessian score less the parent's term; else the parent's term is the minimum score
-    (hessian_split_score_subtract_parent)."""
-    c = np.asarray(cnt, np.float64)[order]
-    cs = np.cumsum(c)
-    ws = None if weight is None else np.cumsum(np.asarray(weight, np.float64)[order])
-    ss = np.cumsum(np.asarray(s, np.float64)[order])
-    hs = np.cumsum(np.asarray(h, np.float64)[order])
-    tc, ts, th = cs[-1], ss[-1], hs[-1]
-    nn, npos = cs[:-1], tc - cs[:-1]
-    valid = (nn >= min_obs) & (npos >= min_obs)
-    with np.errstate(invalid="ignore", divide="ignore"):
-        if not use_hessian:
-            c0, wn, wp = (tc, nn, npos) if ws is None else (ws[-1], ws[:-1], ws[-1] - ws[:-1])
-            valid &= (wn > 0) & (wp > 0)
-            d = (ts - ss[:-1]) * wn - ss[:-1] * wp
-            sc = (d / wp) * (d / wn) / (c0 * c0)
-            valid &= sc > 0
-        else:
-            parent = ts * ts / (max(th, MIN_HESSIAN) + l2_categorical)
-            gn, gp = ss[:-1], ts - ss[:-1]
-            hn = np.maximum(hs[:-1], MIN_HESSIAN) + l2_categorical
-            hp = np.maximum(th - hs[:-1], MIN_HESSIAN) + l2_categorical
-            sc = gp * gp / hp + gn * gn / hn - (parent if subtract_parent else 0.0)
-            valid &= sc > (0.0 if subtract_parent else parent)
-    return np.where(valid, sc, -1.0), npos
 
 
 def best_split(cnt, s, h, use_hessian, min_obs=1, l2_categorical=1.0, weight=None, subtract_parent=False):

@@ -44,6 +44,13 @@ FEATURE_DISCRETIZED_NUMERICAL = 0
 FEATURE_CATEGORICAL = 1
 FEATURE_NUMERICAL = 2   # presorted numerical column (Dataset.set_numerical_column)
 
+LEVEL_NODE_DTYPE = np.dtype([("node", "<i4"), ("candidate", "<i4"), ("derived", "<i4"), ("reserved", "<i4"),
+                             ("num_examples", "<i8")])
+assert LEVEL_NODE_DTYPE.itemsize == 24  # sizeof(ygg_level_node)
+CANDIDATE_DTYPE = np.dtype([("found", "<i4"), ("score", "<f4"), ("threshold_bin", "<i4"), ("lo", "<i4"), ("hi", "<i4"),
+                            ("num_pos_examples", "<i4"), ("threshold_value", "<f4"), ("cat_mask", "<u4", (8,))])
+assert CANDIDATE_DTYPE.itemsize == 60  # sizeof(ygg_candidate)
+
 HIST_ROOT_SUM, HIST_PACKED, HIST_SHARED, HIST2, HIST_SEGMENTED = 0, 1, 2, 3, 4   # enum ygg_hist_mode
 
 
@@ -81,6 +88,7 @@ EXPORTS = [
     "ygg_dataset_set_wide_column", "ygg_dataset_get_wide_column", "ygg_debug_wide_histogram",
     "ygg_dataset_set_wide_categorical_column", "ygg_gbt_get_category_set",
     "ygg_dataset_set_numerical_column", "ygg_dataset_get_numerical_column",
+    "ygg_debug_capture_candidates", "ygg_debug_level_candidates",
 ]
 
 
@@ -708,6 +716,37 @@ class Gbt:
         cnt = c[0, feature - lo, :nb].astype(np.int64)
         raw = s[0, feature - lo, :nb].astype(np.int64) - cnt * 2 ** 23   # exact: |raw| <= rows * 2^23 < 2^63
         return raw.astype(np.float64) * (P / 2.0 ** 23), cnt
+
+    def capture_candidates(self, on=True):
+        """Candidate capture (ygg_debug_capture_candidates): while on, every tree grown copies each level's complete
+        candidate table as the scan phase left it, before the selection."""
+        check(lib().ygg_debug_capture_candidates(self.handle, C.c_int32(int(bool(on)))))
+
+    def level_candidates(self, level):
+        """The captured candidates of tree level `level` of the last tree grown with capture on, as a dict of numpy arrays:
+        per level node `node` (pre-order index in the emitted tree), `candidate`, `derived`, `num_examples`; per (level node,
+        feature scanned by this handle) `found`, `score`, `threshold_bin`, `lo` / `hi` (-1 unless packed by the exact
+        rule), `num_pos_examples`, `threshold_value`, `cat_mask` [.., 8] and, with wide categorical columns, `sets`
+        [nodes, wide features, words]; and the tree's scales `P`, `h_pow2`, `w_pow2`."""
+        cap = 1 << max(0, self.cfg.max_depth - 1)
+        lo, hi = self.hist_features()
+        nodes = np.zeros(cap, LEVEL_NODE_DTYPE)
+        cands = np.zeros((cap, hi - lo), CANDIDATE_DTYPE)
+        wide = getattr(self.dataset, "wide", {})
+        words = max([(nb + 31) // 32 for f, (nb, _) in wide.items()
+                     if self.dataset.feature_types[f] == FEATURE_CATEGORICAL] or [0])
+        sets = np.zeros((cap, len(wide), words), np.uint32) if words else None
+        n, scales = C.c_int32(), np.zeros(3, np.float32)
+        check(lib().ygg_debug_level_candidates(self.handle, C.c_int32(int(level)), C.c_int32(cap),
+                                               nodes.ctypes.data_as(C.c_void_p), cands.ctypes.data_as(C.c_void_p),
+                                               ptr(sets, C.c_uint32), C.c_int32(words), C.byref(n), ptr(scales, C.c_float)))
+        k = n.value
+        out = {name: nodes[name][:k].copy() for name in ("node", "candidate", "derived", "num_examples")}
+        out.update({name: cands[name][:k].copy() for name in CANDIDATE_DTYPE.names})
+        if sets is not None:
+            out["sets"] = sets[:k].copy()
+        out["P"], out["h_pow2"], out["w_pow2"] = (float(x) for x in scales)
+        return out
 
     def hist_features(self):
         """[begin, end) of the features this handle histograms (its feature shard, or all features)."""

@@ -213,6 +213,23 @@ struct ygg_gbt {
   bool scratch_tree = false;         // d_nodes_scratch holds the tree of the last ygg_tree_train_on_gradients call
   ShardBest* d_shard_best = nullptr;
   TieRec* d_ties = nullptr;        // [max level nodes] ties of the level being selected (single GPU)
+  // split-candidate capture (ygg_debug_capture_candidates): per level of the last tree, [num_levels] copies of the scan
+  // phase's tables (d_cand, d_cand_mask, d_wide_thr, d_wide_set), of the node table, the level's families and descriptor
+  struct Capture {
+    bool on = false;
+    int levels = 0;                   // levels captured of the last tree (0: none yet)
+    const NodeRec* tree = nullptr;    // its node table
+    int f_scan = 0;
+    size_t nodes = 0, set_elems = 0;  // per level: split-level nodes, positive-set words
+    Candidate* cand = nullptr;
+    uint32_t* mask = nullptr;
+    float* thr = nullptr;
+    uint32_t* set = nullptr;
+    NodeRec* node_tab = nullptr;      // [num_levels][max_nodes]
+    Family* fam = nullptr;            // [num_levels][max_level_nodes]
+    LevelDesc* lv = nullptr;          // [num_levels]
+    DeviceState* st = nullptr;        // the tree's scales (P, h_pow2), as its levels were scanned
+  } cap;
   // stochastic gradient boosting (cfg.subsample < 1): this iteration's sample, drawn on the host from the learner's engine
   uint8_t* d_selected = nullptr;   // [n_pad]
   std::vector<uint8_t> host_selected;
@@ -1161,6 +1178,35 @@ int launch_weight_sums(ygg_gbt* h, NodeRec* nodes) {
   return check_launch("k_weight_sums");
 }
 
+void free_capture(ygg_gbt* h) {
+  dev_free(h->cap.cand); dev_free(h->cap.mask); dev_free(h->cap.thr); dev_free(h->cap.set);
+  dev_free(h->cap.node_tab); dev_free(h->cap.fam); dev_free(h->cap.lv); dev_free(h->cap.st);
+  h->cap = ygg_gbt::Capture{};
+}
+
+// Copies level l's candidate tables as the scan phase left them (before k_select_local) into the capture buffers;
+// asynchronous, on the handle's stream.
+int capture_level(ygg_gbt* h, int l, const NodeRec* nodes, int par) {
+  ygg_gbt::Capture& c = h->cap;
+  if (c.f_scan != h->f_end - h->f_begin)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "the feature shard changed after ygg_debug_capture_candidates");
+  const size_t per = c.nodes * c.f_scan;
+  auto copy = [&](void* dst, const void* src, size_t bytes) {
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, h->stream);
+  };
+  YGG_CUDA(copy(c.cand + l * per, h->d_cand, per * sizeof(Candidate)));
+  YGG_CUDA(copy(c.mask + l * per * 8, h->d_cand_mask, per * 8 * sizeof(uint32_t)));
+  if (c.thr != nullptr) YGG_CUDA(copy(c.thr + l * per, h->d_wide_thr, per * sizeof(float)));
+  if (c.set != nullptr) YGG_CUDA(copy(c.set + l * c.set_elems, h->d_wide_set, c.set_elems * sizeof(uint32_t)));
+  YGG_CUDA(copy(c.node_tab + static_cast<size_t>(l) * h->max_nodes, nodes, h->max_nodes * sizeof(NodeRec)));
+  YGG_CUDA(copy(c.fam + static_cast<size_t>(l) * h->max_level_nodes, h->d_fam[par], h->max_level_nodes * sizeof(Family)));
+  YGG_CUDA(copy(c.lv + l, h->d_levels + l, sizeof(LevelDesc)));
+  YGG_CUDA(copy(c.st, h->d_st, sizeof(DeviceState)));
+  c.tree = nodes;
+  c.levels = l + 1;
+  return YGG_OK;
+}
+
 // Grows one tree on the gradients currently in d_g / d_h (gmax_bits must already be in d_st and the
 // iteration scalars reset).  Everything is enqueued on h->stream; no host sync.
 //
@@ -1312,6 +1358,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
         YGG_RETURN_IF_ERROR(presort_scan(h, presort_params(h, nodes, l, sc)));
       }
     }
+    if (h->cap.on) YGG_RETURN_IF_ERROR(capture_level(h, l, nodes, par));
     {
       ProfScope ps(h, "select");
       SelectParams sel{};
@@ -2615,6 +2662,7 @@ int ygg_gbt_destroy(ygg_gbt* h) {
   dev_free(h->d_master_val); dev_free(h->d_master_row); dev_free(h->d_ps); dev_free(h->d_ph); dev_free(h->d_presort_temp);
   for (int i = 0; i < 2; i++) { dev_free(h->d_list_val[i]); dev_free(h->d_list_row[i]); }
   dev_free(h->d_seg_off); dev_free(h->d_seg_total); dev_free(h->d_sbest); dev_free(h->d_sbest_idx); dev_free(h->d_num_feature);
+  free_capture(h);
   cudaFree(h->d_goss_temp);
   cudaFree(h->d_level_buf);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -3626,6 +3674,120 @@ int ygg_debug_wide_histogram(ygg_gbt* h, int32_t n_slots, uint64_t* out_sum, uin
   YGG_CUDA(cudaMemcpyAsync(out_cnt, h->d_wcnt, elems * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   if (hh) YGG_CUDA(cudaMemcpyAsync(out_second, h->d_whsum, elems * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
   YGG_CUDA(cudaStreamSynchronize(h->stream));
+  return YGG_OK;
+}
+
+int ygg_debug_capture_candidates(ygg_gbt* h, int32_t enabled) {
+  if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
+  // (both rewrite the finished tree: its splits are no longer the level loop's choices)
+  if (enabled && (h->cfg.candidate_shuffle != 0 || h->cfg.growing_strategy != 0))
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "candidate capture covers level-wise trees without the tie-break replay");
+  YGG_CUDA(cudaSetDevice(h->ds->device));
+  YGG_CUDA(cudaStreamSynchronize(h->stream));   // no copy of a capture being freed is in flight
+  free_capture(h);
+  if (!enabled || h->num_levels == 0) {
+    h->cap.on = enabled != 0;
+    return YGG_OK;
+  }
+  ygg_gbt::Capture& c = h->cap;
+  const size_t L = static_cast<size_t>(h->num_levels);
+  c.f_scan = h->f_end - h->f_begin;
+  c.nodes = static_cast<size_t>(1) << std::max(0, h->num_levels - 1);   // = allocate_level_buffers' split-level nodes
+  const size_t per = c.nodes * c.f_scan;
+  int st = dev_alloc(&c.cand, L * per);
+  if (st == YGG_OK) st = dev_alloc(&c.mask, L * per * 8);
+  if (st == YGG_OK && h->d_wide_thr != nullptr) st = dev_alloc(&c.thr, L * per);
+  if (st == YGG_OK && h->d_wide_set != nullptr) {
+    c.set_elems = c.nodes * h->ds->n_wide() * h->set_words;
+    st = dev_alloc(&c.set, L * c.set_elems);
+  }
+  if (st == YGG_OK) st = dev_alloc(&c.node_tab, L * h->max_nodes);
+  if (st == YGG_OK) st = dev_alloc(&c.fam, L * h->max_level_nodes);
+  if (st == YGG_OK) st = dev_alloc(&c.lv, L);
+  if (st == YGG_OK) st = dev_alloc(&c.st, 1);
+  if (st != YGG_OK) {
+    free_capture(h);
+    return st;
+  }
+  c.on = true;
+  return YGG_OK;
+}
+
+int ygg_debug_level_candidates(ygg_gbt* h, int32_t level, int32_t capacity, ygg_level_node* nodes_out, ygg_candidate* cands,
+                               uint32_t* sets, int32_t set_words, int32_t* n_nodes, float* scales) {
+  if (!h || !nodes_out || !cands || !n_nodes || !scales) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  const ygg_gbt::Capture& c = h->cap;
+  if (!c.on) return set_error(YGG_ERR_INVALID_ARGUMENT, "candidate capture is not enabled (ygg_debug_capture_candidates)");
+  if (c.levels == 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "no tree was grown since candidate capture was enabled");
+  if (level < 0 || level >= c.levels) return set_error(YGG_ERR_INVALID_ARGUMENT, "level %d outside [0, %d)", level, c.levels);
+  if (sets != nullptr && set_words != h->set_words)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "set_words=%d, the handle's positive sets have %d words", set_words, h->set_words);
+  const ygg_dataset* ds = h->ds;
+  YGG_CUDA(cudaSetDevice(ds->device));
+  const size_t per = c.nodes * c.f_scan;
+  LevelDesc lv{};
+  DeviceState dst{};
+  std::vector<NodeRec> tab(h->max_nodes), tree(h->max_nodes);
+  std::vector<Family> fam(h->max_level_nodes);
+  std::vector<Candidate> cand(per);
+  std::vector<uint32_t> mask(per * 8), set(c.set ? c.set_elems : 0);
+  std::vector<float> thr(c.thr ? per : 0), bucket_values(ds->d_bucket_values ? static_cast<size_t>(ds->F) * kMaxBins : 0);
+  auto get = [&](void* dst_, const void* src, size_t bytes) {
+    return cudaMemcpyAsync(dst_, src, bytes, cudaMemcpyDeviceToHost, h->stream);
+  };
+  YGG_CUDA(get(&lv, c.lv + level, sizeof(LevelDesc)));
+  YGG_CUDA(get(&dst, c.st, sizeof(DeviceState)));
+  YGG_CUDA(get(tab.data(), c.node_tab + static_cast<size_t>(level) * h->max_nodes, tab.size() * sizeof(NodeRec)));
+  YGG_CUDA(get(tree.data(), c.tree, tree.size() * sizeof(NodeRec)));
+  YGG_CUDA(get(fam.data(), c.fam + static_cast<size_t>(level) * h->max_level_nodes, fam.size() * sizeof(Family)));
+  YGG_CUDA(get(cand.data(), c.cand + level * per, per * sizeof(Candidate)));
+  YGG_CUDA(get(mask.data(), c.mask + level * per * 8, per * 8 * sizeof(uint32_t)));
+  if (c.thr) YGG_CUDA(get(thr.data(), c.thr + level * per, per * sizeof(float)));
+  if (c.set) YGG_CUDA(get(set.data(), c.set + level * c.set_elems, c.set_elems * sizeof(uint32_t)));
+  if (!bucket_values.empty()) YGG_CUDA(get(bucket_values.data(), ds->d_bucket_values, bucket_values.size() * sizeof(float)));
+  YGG_CUDA(cudaStreamSynchronize(h->stream));
+  *n_nodes = lv.num_nodes;
+  if (lv.num_nodes > capacity) return set_error(YGG_ERR_INVALID_ARGUMENT, "capacity %d < %d level nodes", capacity, lv.num_nodes);
+  std::vector<int> ids, pre(h->max_nodes, -1);
+  preorder_ids(tree, 0, &ids);
+  for (size_t i = 0; i < ids.size(); i++) pre[ids[i]] = static_cast<int>(i);
+  std::vector<int> derived(lv.num_nodes, 0);
+  for (int f = 0; f < lv.num_families; f++)
+    if (fam[f].derived >= 0) derived[fam[f].derived - lv.first_node] = 1;
+  for (int j = 0; j < lv.num_nodes; j++) {
+    const NodeRec& nd = tab[lv.first_node + j];
+    nodes_out[j] = ygg_level_node{pre[lv.first_node + j], nd.candidate, derived[j], 0, nd.n};
+    for (int fl = 0; fl < c.f_scan; fl++) {
+      const size_t ci = static_cast<size_t>(j) * c.f_scan + fl;
+      const int fg = h->f_begin + fl;
+      const Candidate& k = cand[ci];
+      ygg_candidate o{};
+      o.lo = o.hi = -1;
+      o.threshold_value = std::numeric_limits<float>::quiet_NaN();
+      if (nd.candidate && k.found) {
+        o.found = 1;
+        o.score = k.score;
+        o.threshold_bin = thr_bin_of(k.thr);
+        o.num_pos_examples = k.n_pos;
+        if (k.thr & kThrExactFlag) {
+          o.lo = (k.thr >> 9) & 0xFF;
+          o.hi = (k.thr >> 17) & 0x1FF;
+          o.threshold_value = thr_value_of(k.thr, bucket_values.data() + static_cast<size_t>(fg) * kMaxBins);
+        }
+        if (!thr.empty() && ((ds->n_wide() > 0 && ds->wide_of[fg] >= 0) || ds->feature_type[fg] == YGG_FEATURE_NUMERICAL))
+          o.threshold_value = thr[ci];
+        for (int i = 0; i < 8; i++) o.cat_mask[i] = mask[ci * 8 + i];
+      }
+      cands[ci] = o;
+    }
+    if (sets != nullptr && c.set != nullptr) {
+      const size_t row = static_cast<size_t>(ds->n_wide()) * h->set_words;
+      for (size_t i = 0; i < row; i++) sets[j * row + i] = nd.candidate ? set[j * row + i] : 0u;
+    }
+  }
+  scales[0] = dst.g_pow2;
+  scales[1] = dst.h_pow2;
+  scales[2] = h->w_pow2;
   return YGG_OK;
 }
 

@@ -417,7 +417,9 @@ __device__ __forceinline__ bool boundary_score(const ScanParams& p, const Scan3&
     // splitter_accumulator.h:1517-1519).  With consistent sums the sum-of-squares terms cancel and
     // the numerator is the between-group sum of squares n_pos*n_neg/c0 * (mean_pos - mean_neg)^2,
     // evaluated from the integer sums as d^2 / (n_pos*n_neg*c0) with d = S_pos*n_neg - S_neg*n_pos:
-    // non-negative by construction and exactly 0 for equal means (DESIGN.md §5).
+    // non-negative by construction and exactly 0 for equal means (DESIGN.md §5).  d is formed in 128-bit integers
+    // (|d| < 2^110) and rounded once: in doubles the two products exceed 2^53 on nodes of ~10^5 rows, and their
+    // rounding (or a contraction of the difference into an FMA) would leave a non-zero d on a pure node.
     double c0 = static_cast<double>(tot.c);
     double np_ = static_cast<double>(n_pos), nn_ = static_cast<double>(n_neg);
     if (p.weighted) {   // weight sums instead of counts (exact integers in units of w_inv)
@@ -427,7 +429,11 @@ __device__ __forceinline__ bool boundary_score(const ScanParams& p, const Scan3&
       valid = valid && np_ > 0.0 && nn_ > 0.0;
     }
     if (valid) {
-      double dq = static_cast<double>(tot.s - inc.s) * nn_ - static_cast<double>(inc.s) * np_;
+      const long long s_pos = tot.s - inc.s, s_neg = inc.s;
+      const long long w_pos = p.weighted ? tot.h - inc.h : n_pos, w_neg = p.weighted ? inc.h : n_neg;
+      // (w_inv is a power of two: the product is exact)
+      double dq = static_cast<double>(static_cast<__int128>(s_pos) * w_neg - static_cast<__int128>(s_neg) * w_pos) *
+                  (p.weighted ? p.w_inv : 1.0);
       if (p.weighted) {
         // Every sum is a sum of ROUNDED products (w*g and w at 2^-24 of their scales), so a node whose rows all carry the
         // same gradient gives d = 0 only up to +-half a unit per row: below that bound d is not distinguishable from 0 and
@@ -569,7 +575,6 @@ __device__ void scan_node_categorical(const ScanParams& p, const NodeRec& node, 
   const int B = p.num_bins[f_global];
   const double ginv = static_cast<double>(p.st->g_pow2) / static_cast<double>(1u << (kQBits - 1));
   const double hinv = static_cast<double>(p.st->h_pow2) / static_cast<double>(1u << kQBits);
-  const double l2 = p.l2_categorical;
   const double key = b >= B ? __longlong_as_double(0x7FF0000000000000ll)   // +inf: not a category of this feature
                             : category_key(p, cnt, sq, hq, ginv, hinv);
   s_key[b] = key; s_idx[b] = b; s_cnt[b] = cnt; s_sq[b] = sq; s_hq[b] = hq;
@@ -592,47 +597,11 @@ __device__ void scan_node_categorical(const ScanParams& p, const NodeRec& node, 
   const int my = s_idx[b];  // category at sorted position b
   Scan3 tot;
   const Scan3 inc = block_inclusive_scan(Scan3{s_cnt[my], s_sq[my], s_hq[my]}, s_warp, &tot);
-  const long long n_neg = inc.c, n_pos = tot.c - inc.c;
-  bool valid = (b <= B - 2) && (n_pos >= p.min_num_obs) && (n_neg >= p.min_num_obs);
-  double score = 0.0, min_score = 0.0;
-  if (!p.use_hessian) {
-    double c0 = static_cast<double>(tot.c);
-    double np_ = static_cast<double>(n_pos), nn_ = static_cast<double>(n_neg);
-    if (p.weighted) {   // weight sums instead of counts (exact integers in units of w_inv)
-      c0 = static_cast<double>(tot.h) * p.w_inv;
-      np_ = static_cast<double>(tot.h - inc.h) * p.w_inv;
-      nn_ = static_cast<double>(inc.h) * p.w_inv;
-      valid = valid && np_ > 0.0 && nn_ > 0.0;
-    }
-    if (valid) {
-      double dq = static_cast<double>(tot.s - inc.s) * nn_ - static_cast<double>(inc.s) * np_;
-      if (p.weighted) {
-        // Every sum is a sum of ROUNDED products (w*g and w at 2^-24 of their scales), so a node whose rows all carry the
-        // same gradient gives d = 0 only up to +-half a unit per row: below that bound d is not distinguishable from 0 and
-        // the split would be decided by rounding (the reference's doubles flip the same coin at 1e-16).  Unweighted sums
-        // are exact integers and need no such floor.
-        const double half_units = 0.5 * (static_cast<double>(n_pos) * nn_ + static_cast<double>(n_neg) * np_ +
-                                         (fabs(static_cast<double>(tot.s - inc.s)) * static_cast<double>(n_neg) +
-                                          fabs(static_cast<double>(inc.s)) * static_cast<double>(n_pos)) * p.w_inv);
-        if (fabs(dq) <= half_units) dq = 0.0;
-      }
-      const double d = dq * ginv;
-      score = (d / np_) * (d / nn_) / (c0 * c0);
-    }
-  } else {
-    const double g0 = l1_threshold_d(static_cast<double>(tot.s) * ginv, p.l1);   // see scan_node
-    const double parent_full = g0 * g0 / (fmax(static_cast<double>(tot.h) * hinv, kMinHessianForNewtonStep) + l2);
-    const double parent_score = p.subtract_parent ? parent_full : 0.0;
-    min_score = p.subtract_parent ? 0.0 : parent_full;
-    if (valid) {
-      const double gn = l1_threshold_d(static_cast<double>(inc.s) * ginv, p.l1);
-      const double gp = l1_threshold_d(static_cast<double>(tot.s - inc.s) * ginv, p.l1);
-      const double hn = fmax(static_cast<double>(inc.h) * hinv, kMinHessianForNewtonStep) + l2;
-      const double hp = fmax(static_cast<double>(tot.h - inc.h) * hinv, kMinHessianForNewtonStep) + l2;
-      score = gp * gp / hp + gn * gn / hn - parent_score;
-    }
-  }
-  valid = valid && (score > min_score) && (score > 0.0 || p.use_hessian);
+  const long long n_pos = tot.c - inc.c;
+  ScanParams sp = p;
+  sp.l2 = p.l2_categorical;
+  double score;
+  const bool valid = boundary_score(sp, tot, inc, b <= B - 2, ginv, hinv, &score);
   double bs = valid ? score : -1.0;
   int bb = valid ? b : 0x7fffffff;
 #pragma unroll
@@ -1407,8 +1376,12 @@ __global__ void k_node_stats(StatsParams p) {
         const double Sn = (static_cast<double>(static_cast<long long>(sg_n)) - nn_ * static_cast<double>(kSBias)) * ginv;
         double score;
         if (!p.use_hessian) {
+          // exact numerator, as in boundary_score: the biases cancel, d = (sg_pos*n_neg - sg_neg*n_pos) * ginv
+          const long long sg_pos = static_cast<long long>(nd.sg) - nd.n * static_cast<long long>(kSBias);
+          const long long sg_neg = static_cast<long long>(sg_n) - sib.n * static_cast<long long>(kSBias);
           const double c0 = np_ + nn_;
-          const double d = Sp * nn_ - Sn * np_;
+          const double d =
+              static_cast<double>(static_cast<__int128>(sg_pos) * sib.n - static_cast<__int128>(sg_neg) * nd.n) * ginv;
           score = (d / np_) * (d / nn_) / (c0 * c0);
         } else {
           const double l2 = par.cond_type == 1 ? p.l2_categorical : p.l2;
