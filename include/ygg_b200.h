@@ -363,6 +363,37 @@ int ygg_gbt_tie_stats(ygg_gbt* h, int64_t* renamed, int64_t* unresolved);
  * decision_tree::Train seam), whose trees are not grown in the handle's own boosting loop. */
 int ygg_gbt_set_tie_rng_position(ygg_gbt* h, uint64_t words);
 
+/* Candidate feature sampling (DecisionTreeTrainingConfig.num_candidate_attributes / num_candidate_attributes_ratio,
+ * decision_tree.proto; DESIGN.md §23): each node is split on the best of a random subset of the features.
+ *
+ * k, the number of features to test (NumAttributesToTest, training.cc:4244-4289), for F features:
+ *   k = ceil(ratio * F) if ratio >= 0 (the product in float arithmetic), else num_candidate_attributes;  k == 0 -> ceil(sqrt(F)) for the binomial and
+ *   multinomial losses, ceil(F / 3) for squared error;  k == -1 -> F;  then k = min(k, F).
+ * ygg_num_candidate_attributes computes it; INVALID_ARGUMENT for num_candidate_attributes < -1, a ratio above 1 or NaN
+ * (a negative ratio means "not set"), F < 1 or an unknown loss.
+ *
+ * Candidate order: the features of node `node` (its index in the handle's node table of the tree) of tree `tree` (the
+ * index ygg_gbt_get_tree takes: iteration * K + class) are ordered by ascending (key, feature) with
+ *   mix(z)  = SplitMix64's finalizer: z += 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+ *             z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31)      (all modulo 2^64)
+ *   key     = mix(mix(mix(mix(random_seed) ^ (uint32)tree) ^ (uint32)node) ^ (uint32)feature)
+ * (ygg_candidate_key).  The order depends on the node alone, not on the order in which nodes are searched, so it draws
+ * nothing from the learner's random stream (row sampling and GOSS are unaffected) and works with every growth strategy.
+ *
+ * Selection: features are taken in that order until k of them (k + 1 with split_jobs_draw_seeds = 0, the reference's
+ * single-thread manager, training.cc:1407) are valid — the scan scored at least one of their boundaries: two non-empty
+ * sides of at least min_examples rows (with in_split_min_examples_check), with or without example weight — or every
+ * feature is taken; the node's split is
+ * the first maximum, by float score, of the taken features in that order.
+ *
+ * ygg_gbt_set_candidate_sampling: after ygg_gbt_create, before the first tree; k >= F keeps the unsampled selection (and
+ * the tie-break replay).  With k < F: YGG_ERR_UNIMPLEMENTED on a feature or row shard (either call order: the shard
+ * setters refuse a sampling handle), INVALID_ARGUMENT with candidate_shuffle != 0 (the keys define the order). */
+int ygg_num_candidate_attributes(int32_t num_features, int32_t loss, int32_t num_candidate_attributes,
+                                 float num_candidate_attributes_ratio, int32_t* k);
+uint64_t ygg_candidate_key(uint32_t random_seed, int32_t tree, int32_t node, int32_t feature);
+int ygg_gbt_set_candidate_sampling(ygg_gbt* h, int32_t num_candidate_attributes, float num_candidate_attributes_ratio);
+
 /* Copies tree `iter` (pre-order: node, neg subtree, pos subtree).  *n_nodes receives the node
  * count; fails with INVALID_ARGUMENT if capacity is too small. */
 int ygg_gbt_get_tree(ygg_gbt* h, int32_t iter, ygg_node* out, int32_t capacity, int32_t* n_nodes);
@@ -464,6 +495,11 @@ typedef struct ygg_candidate {
  * output, a level outside the captured tree, a capacity below the level's nodes or no capture. */
 int ygg_debug_level_candidates(ygg_gbt* h, int32_t level, int32_t capacity, ygg_level_node* nodes, ygg_candidate* cands,
                                uint32_t* sets, int32_t set_words, int32_t* n_nodes, float* scales);
+/* The candidate feature sampling validity flags of the same capture (sampling set before the capture was enabled):
+ * tried[capacity][features] = 1 when the scan scored at least one boundary of the (level node, feature) pair, 0 otherwise
+ * and on nodes that were not scanned; *first_node = the node-table index of the level's first node (level node j is
+ * node first_node + j of ygg_candidate_key).  INVALID_ARGUMENT as ygg_debug_level_candidates, or without sampling. */
+int ygg_debug_level_tried(ygg_gbt* h, int32_t level, int32_t capacity, uint8_t* tried, int32_t* first_node, int32_t* n_nodes);
 
 /* SplitExamplesInPlace seam (learner/decision_tree/training.cc:5243-5305 ->
  * model/decision_tree/decision_tree.cc:957-1012): stable two-way partition of a row-id list by

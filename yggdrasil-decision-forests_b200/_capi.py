@@ -89,6 +89,7 @@ EXPORTS = [
     "ygg_dataset_set_wide_categorical_column", "ygg_gbt_get_category_set",
     "ygg_dataset_set_numerical_column", "ygg_dataset_get_numerical_column",
     "ygg_debug_capture_candidates", "ygg_debug_level_candidates",
+    "ygg_num_candidate_attributes", "ygg_candidate_key", "ygg_gbt_set_candidate_sampling", "ygg_debug_level_tried",
 ]
 
 
@@ -102,6 +103,8 @@ def lib():
         L.ygg_last_error.restype = C.c_char_p
         L.ygg_dataset_num_rows.restype = C.c_int64
         L.ygg_gbt_config_init.restype = None
+        L.ygg_candidate_key.restype = C.c_uint64
+        L.ygg_candidate_key.argtypes = [C.c_uint32, C.c_int32, C.c_int32, C.c_int32]
         for name in EXPORTS:
             getattr(L, name)  # fail loudly on a missing symbol
         _LIB = L
@@ -115,6 +118,21 @@ def check(status):
 
 def ptr(a, t):
     return a.ctypes.data_as(C.POINTER(t)) if a is not None else None
+
+
+def num_candidate_attributes(num_features, loss, num_candidate_attributes=-1, ratio=None):
+    """k, the number of features a node tests under candidate feature sampling (ygg_num_candidate_attributes); ratio None
+    (or negative): not set."""
+    k = C.c_int32()
+    check(lib().ygg_num_candidate_attributes(C.c_int32(int(num_features)), C.c_int32(int(loss)),
+                                             C.c_int32(int(num_candidate_attributes)),
+                                             C.c_float(-1.0 if ratio is None else float(ratio)), C.byref(k)))
+    return k.value
+
+
+def candidate_key(seed, tree, node, feature):
+    """The key ordering `feature` among the candidates of node `node` of tree `tree` (ygg_candidate_key)."""
+    return int(lib().ygg_candidate_key(int(seed) & 0xFFFFFFFF, int(tree), int(node), int(feature)))
 
 
 def default_config(**kw):
@@ -716,6 +734,23 @@ class Gbt:
         cnt = c[0, feature - lo, :nb].astype(np.int64)
         raw = s[0, feature - lo, :nb].astype(np.int64) - cnt * 2 ** 23   # exact: |raw| <= rows * 2^23 < 2^63
         return raw.astype(np.float64) * (P / 2.0 ** 23), cnt
+
+    def set_candidate_sampling(self, num_candidate_attributes=-1, ratio=None):
+        """Candidate feature sampling (ygg_gbt_set_candidate_sampling): each node tests the first k valid features of its
+        keyed order; ratio None: not set.  Before the first tree."""
+        check(lib().ygg_gbt_set_candidate_sampling(self.handle, C.c_int32(int(num_candidate_attributes)),
+                                                   C.c_float(-1.0 if ratio is None else float(ratio))))
+
+    def level_tried(self, level):
+        """The validity flags of tree level `level` of the last captured tree (sampling set before capture_candidates):
+        (tried uint8 [level nodes, features scanned by this handle], node-table index of the level's first node)."""
+        cap = 1 << max(0, self.cfg.max_depth - 1)
+        lo, hi = self.hist_features()
+        out = np.zeros((cap, hi - lo), np.uint8)
+        first, n = C.c_int32(), C.c_int32()
+        check(lib().ygg_debug_level_tried(self.handle, C.c_int32(int(level)), C.c_int32(cap), ptr(out, C.c_uint8),
+                                          C.byref(first), C.byref(n)))
+        return out[:n.value].copy(), first.value
 
     def capture_candidates(self, on=True):
         """Candidate capture (ygg_debug_capture_candidates): while on, every tree grown copies each level's complete

@@ -136,6 +136,28 @@ inline ShardBest merge_shard_bests(const ShardBest* records, int world, int stri
   return best;
 }
 
+// Candidate feature sampling (DESIGN.md §23): the key that orders feature f among the candidates of node `node` (its place
+// in the tree's node table) of tree `tree` (iteration * K + class).  Chained SplitMix64 finalizers; the candidate order of a
+// node is ascending (key, f).  Restated in include/ygg_b200.h (ygg_candidate_key).
+#ifdef __CUDACC__
+__host__ __device__
+#endif
+inline uint64_t splitmix64_mix(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+#ifdef __CUDACC__
+__host__ __device__
+#endif
+inline uint64_t candidate_key(uint32_t seed, int32_t tree, int32_t node, int32_t f) {
+  uint64_t z = splitmix64_mix(seed);
+  z = splitmix64_mix(z ^ static_cast<uint32_t>(tree));
+  z = splitmix64_mix(z ^ static_cast<uint32_t>(node));
+  return splitmix64_mix(z ^ static_cast<uint32_t>(f));
+}
+
 // Scalars living in device memory so the level loop never syncs with the host.
 struct DeviceState {
   float g_pow2;        // P: power of two > max|g| (histogram + statistics scale of g)

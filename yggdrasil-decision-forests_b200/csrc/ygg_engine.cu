@@ -213,6 +213,10 @@ struct ygg_gbt {
   bool scratch_tree = false;         // d_nodes_scratch holds the tree of the last ygg_tree_train_on_gradients call
   ShardBest* d_shard_best = nullptr;
   TieRec* d_ties = nullptr;        // [max level nodes] ties of the level being selected (single GPU)
+  // candidate feature sampling (ygg_gbt_set_candidate_sampling, DESIGN.md §23): valid features tested per node (k, or k + 1
+  // with the single-thread manager; 0: off), the scan's validity flags [split-level nodes][f_scan]
+  int sample_k_valid = 0;
+  uint8_t* d_tried = nullptr;
   // split-candidate capture (ygg_debug_capture_candidates): per level of the last tree, [num_levels] copies of the scan
   // phase's tables (d_cand, d_cand_mask, d_wide_thr, d_wide_set), of the node table, the level's families and descriptor
   struct Capture {
@@ -225,6 +229,7 @@ struct ygg_gbt {
     uint32_t* mask = nullptr;
     float* thr = nullptr;
     uint32_t* set = nullptr;
+    uint8_t* tried = nullptr;         // candidate feature sampling's validity flags (null without sampling)
     NodeRec* node_tab = nullptr;      // [num_levels][max_nodes]
     Family* fam = nullptr;            // [num_levels][max_level_nodes]
     LevelDesc* lv = nullptr;          // [num_levels]
@@ -1179,7 +1184,7 @@ int launch_weight_sums(ygg_gbt* h, NodeRec* nodes) {
 }
 
 void free_capture(ygg_gbt* h) {
-  dev_free(h->cap.cand); dev_free(h->cap.mask); dev_free(h->cap.thr); dev_free(h->cap.set);
+  dev_free(h->cap.cand); dev_free(h->cap.mask); dev_free(h->cap.thr); dev_free(h->cap.set); dev_free(h->cap.tried);
   dev_free(h->cap.node_tab); dev_free(h->cap.fam); dev_free(h->cap.lv); dev_free(h->cap.st);
   h->cap = ygg_gbt::Capture{};
 }
@@ -1198,6 +1203,7 @@ int capture_level(ygg_gbt* h, int l, const NodeRec* nodes, int par) {
   YGG_CUDA(copy(c.mask + l * per * 8, h->d_cand_mask, per * 8 * sizeof(uint32_t)));
   if (c.thr != nullptr) YGG_CUDA(copy(c.thr + l * per, h->d_wide_thr, per * sizeof(float)));
   if (c.set != nullptr) YGG_CUDA(copy(c.set + l * c.set_elems, h->d_wide_set, c.set_elems * sizeof(uint32_t)));
+  if (c.tried != nullptr) YGG_CUDA(copy(c.tried + l * per, h->d_tried, per));
   YGG_CUDA(copy(c.node_tab + static_cast<size_t>(l) * h->max_nodes, nodes, h->max_nodes * sizeof(NodeRec)));
   YGG_CUDA(copy(c.fam + static_cast<size_t>(l) * h->max_level_nodes, h->d_fam[par], h->max_level_nodes * sizeof(Family)));
   YGG_CUDA(copy(c.lv + l, h->d_levels + l, sizeof(LevelDesc)));
@@ -1323,6 +1329,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       sc.bucket_values = ds->d_bucket_values; sc.exact_rule = ds->d_exact_rule;
       sc.weighted = weighted(h) ? 1 : 0;
       sc.w_inv = static_cast<double>(h->w_pow2) / static_cast<double>(1u << kQBits);
+      sc.tried = h->sample_k_valid > 0 ? h->d_tried : nullptr;
       dim3 grid(level_slot_bound(h, l), f_count);
       if (hist_hess(h) || use_hess(h)) k_scan<true><<<grid, 256, 0, h->stream>>>(sc);
       else k_scan<false><<<grid, 256, 0, h->stream>>>(sc);
@@ -1377,10 +1384,17 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
       sel.st = h->d_st; sel.max_nodes = h->max_nodes;
       sel.wide_of = h->wide_total > 0 ? ds->d_wide_of : nullptr; sel.wide_thr_value = h->d_wide_thr;
       sel.wide_set = h->d_wide_set; sel.wide_na_bin = h->d_wide_na_bin; sel.n_wide = ds->n_wide(); sel.set_words = h->set_words;
-      const int threads = 256, blocks = (level_nodes_bound + (threads / 32) - 1) / (threads / 32);
-      k_select_local<<<blocks, threads, 0, h->stream>>>(sel);
-      h->launches_total++;
-      YGG_RETURN_IF_ERROR(check_launch("k_select_local"));
+      if (h->sample_k_valid > 0) {
+        SampleParams smp{h->d_tried, h->sample_k_valid, h->cfg.random_seed, h->trees_done};
+        k_select_sampled<<<level_nodes_bound, 256, 0, h->stream>>>(sel, smp);
+        h->launches_total++;
+        YGG_RETURN_IF_ERROR(check_launch("k_select_sampled"));
+      } else {
+        const int threads = 256, blocks = (level_nodes_bound + (threads / 32) - 1) / (threads / 32);
+        k_select_local<<<blocks, threads, 0, h->stream>>>(sel);
+        h->launches_total++;
+        YGG_RETURN_IF_ERROR(check_launch("k_select_local"));
+      }
       sel.peers = nullptr; sel.epoch = 0;
       if (exchange_bests && h->d_peer_windows != nullptr) {
         sel.peers = h->d_peer_windows;   // k_select_global exchanges the records itself over peer memory
@@ -2649,7 +2663,7 @@ int ygg_gbt_destroy(ygg_gbt* h) {
     dev_free(h->d_fam[i]); dev_free(h->d_slot_node[i]); dev_free(h->d_hist_sum[i]); dev_free(h->d_hist_cnt[i]);
     dev_free(h->d_hist_hsum[i]);
   }
-  dev_free(h->d_nodes_all); dev_free(h->d_nodes_scratch); dev_free(h->d_cand); dev_free(h->d_cand_mask); cudaFree(h->d_shard_best); dev_free(h->d_loss); dev_free(h->d_loss_partials); dev_free(h->d_ties); dev_free(h->d_selected); dev_free(h->d_peer_windows);
+  dev_free(h->d_nodes_all); dev_free(h->d_nodes_scratch); dev_free(h->d_cand); dev_free(h->d_cand_mask); cudaFree(h->d_shard_best); dev_free(h->d_loss); dev_free(h->d_loss_partials); dev_free(h->d_ties); dev_free(h->d_tried); dev_free(h->d_selected); dev_free(h->d_peer_windows);
   dev_free(h->d_vpred); dev_free(h->d_vlabel_u8); dev_free(h->d_vlabel_f32); dev_free(h->d_vloss);
   dev_free(h->d_weight); dev_free(h->d_g2w); dev_free(h->d_wsums); dev_free(h->d_vweight);
   for (int i = 0; i < 2; i++) { dev_free(h->d_goss_keys[i]); dev_free(h->d_goss_rows[i]); }
@@ -2869,6 +2883,7 @@ int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature
   if (world > 1 && !exchange) return set_error(YGG_ERR_INVALID_ARGUMENT, "world > 1 needs an exchange function");
   if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "shard must be set before training");
   if (world > 1 && h->cfg.candidate_shuffle != 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate_shuffle is not combined with sharding");
+  if (h->sample_k_valid > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate feature sampling is not combined with sharding");
   YGG_CUDA(cudaSetDevice(h->ds->device));
   h->f_begin = feature_begin; h->f_end = feature_end; h->rank = rank; h->world = world;
   h->hist_f_begin = feature_begin; h->hist_f_end = feature_end;
@@ -2893,6 +2908,7 @@ int ygg_gbt_set_row_shard(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_row
   if (!h->has_labels) return set_error(YGG_ERR_INVALID_ARGUMENT, "set the labels before the row shard");
 
   if (world > 1 && h->cfg.candidate_shuffle != 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate_shuffle is not combined with sharding");
+  if (h->sample_k_valid > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate feature sampling is not combined with sharding");
   if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "shard must be set before training");
   YGG_CUDA(cudaSetDevice(h->ds->device));
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
@@ -3701,6 +3717,7 @@ int ygg_debug_capture_candidates(ygg_gbt* h, int32_t enabled) {
     c.set_elems = c.nodes * h->ds->n_wide() * h->set_words;
     st = dev_alloc(&c.set, L * c.set_elems);
   }
+  if (st == YGG_OK && h->sample_k_valid > 0) st = dev_alloc(&c.tried, L * per);
   if (st == YGG_OK) st = dev_alloc(&c.node_tab, L * h->max_nodes);
   if (st == YGG_OK) st = dev_alloc(&c.fam, L * h->max_level_nodes);
   if (st == YGG_OK) st = dev_alloc(&c.lv, L);
@@ -3862,6 +3879,92 @@ int ygg_gbt_tie_stats(ygg_gbt* h, int64_t* renamed, int64_t* unresolved) {
   YGG_RETURN_IF_ERROR(resolve_ties(h, h->trees_done));
   *renamed = h->ties_renamed;
   *unresolved = h->ties_unresolved;
+  return YGG_OK;
+}
+
+int ygg_num_candidate_attributes(int32_t num_features, int32_t loss, int32_t num_candidate_attributes,
+                                 float num_candidate_attributes_ratio, int32_t* k) {
+  if (!k) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (num_features < 1) return set_error(YGG_ERR_INVALID_ARGUMENT, "num_features=%d", num_features);
+  if (loss < YGG_LOSS_BINOMIAL_LOG_LIKELIHOOD || loss > YGG_LOSS_MULTINOMIAL_LOG_LIKELIHOOD)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "unknown loss %d", loss);
+  if (num_candidate_attributes < -1)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "num_candidate_attributes=%d below -1", num_candidate_attributes);
+  if (std::isnan(num_candidate_attributes_ratio) || num_candidate_attributes_ratio > 1.f)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "num_candidate_attributes_ratio=%g above 1", num_candidate_attributes_ratio);
+  // NumAttributesToTest (training.cc:4244-4289)
+  int n = num_candidate_attributes;
+  // the proto's float ratio times the int count, in float arithmetic, as the reference computes it (training.cc:4259-4260)
+  if (num_candidate_attributes_ratio >= 0.f) {
+    const float product = num_candidate_attributes_ratio * static_cast<float>(num_features);
+    n = static_cast<int>(std::ceil(product));
+  }
+  if (n == 0) {
+    n = loss == YGG_LOSS_SQUARED_ERROR ? static_cast<int>(std::ceil(static_cast<double>(num_features) / 3))
+                                       : static_cast<int>(std::ceil(std::sqrt(static_cast<double>(num_features))));
+  }
+  if (n == -1) n = num_features;
+  *k = std::min(n, num_features);
+  return YGG_OK;
+}
+
+uint64_t ygg_candidate_key(uint32_t random_seed, int32_t tree, int32_t node, int32_t feature) {
+  return candidate_key(random_seed, tree, node, feature);
+}
+
+int ygg_gbt_set_candidate_sampling(ygg_gbt* h, int32_t num_candidate_attributes, float num_candidate_attributes_ratio) {
+  if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
+  if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "candidate sampling must be set before training");
+  int32_t k = 0;
+  YGG_RETURN_IF_ERROR(ygg_num_candidate_attributes(h->ds->F, h->cfg.loss, num_candidate_attributes, num_candidate_attributes_ratio, &k));
+  if (k >= h->ds->F) {   // every feature is tested: the unsampled selection, tie-break replay included
+    h->sample_k_valid = 0;
+    return YGG_OK;
+  }
+  // the "first k valid" cutoff needs the validity of every feature, which no rank of a shard holds
+  if (h->shard_mode != kShardNone || h->f_begin != 0 || h->f_end != h->ds->F)
+    return set_error(YGG_ERR_UNIMPLEMENTED, "candidate feature sampling is not combined with sharding");
+  if (h->cfg.candidate_shuffle != 0)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "candidate feature sampling orders the candidates itself: candidate_shuffle must be 0");
+  if (h->cap.on && h->cap.tried == nullptr)   // the capture's buffers were sized without the flags
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "set candidate sampling before ygg_debug_capture_candidates");
+  YGG_CUDA(cudaSetDevice(h->ds->device));
+  if (h->d_tried == nullptr) {
+    const size_t split_level_nodes = static_cast<size_t>(1) << std::max(0, h->num_levels - 1);
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_tried, split_level_nodes * h->ds->F));
+  }
+  // FindBestConditionSingleThreadManager tests one more valid feature than its concurrent counterpart (training.cc:1407)
+  h->sample_k_valid = h->cfg.split_jobs_draw_seeds != 0 ? k : k + 1;
+  return YGG_OK;
+}
+
+int ygg_debug_level_tried(ygg_gbt* h, int32_t level, int32_t capacity, uint8_t* tried, int32_t* first_node, int32_t* n_nodes) {
+  if (!h || !tried || !first_node || !n_nodes) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  const ygg_gbt::Capture& c = h->cap;
+  if (!c.on || c.tried == nullptr)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "candidate capture with candidate feature sampling is not enabled");
+  if (c.levels == 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "no tree was grown since candidate capture was enabled");
+  if (level < 0 || level >= c.levels) return set_error(YGG_ERR_INVALID_ARGUMENT, "level %d outside [0, %d)", level, c.levels);
+  YGG_CUDA(cudaSetDevice(h->ds->device));
+  LevelDesc lv{};
+  std::vector<NodeRec> tab(h->max_nodes);
+  const size_t per = c.nodes * c.f_scan;
+  std::vector<uint8_t> flags(per);
+  YGG_CUDA(cudaMemcpyAsync(&lv, c.lv + level, sizeof(LevelDesc), cudaMemcpyDeviceToHost, h->stream));
+  YGG_CUDA(cudaMemcpyAsync(tab.data(), c.node_tab + static_cast<size_t>(level) * h->max_nodes, tab.size() * sizeof(NodeRec),
+                           cudaMemcpyDeviceToHost, h->stream));
+  YGG_CUDA(cudaMemcpyAsync(flags.data(), c.tried + level * per, per, cudaMemcpyDeviceToHost, h->stream));
+  YGG_CUDA(cudaStreamSynchronize(h->stream));
+  *n_nodes = lv.num_nodes;
+  *first_node = lv.first_node;
+  if (lv.num_nodes > capacity) return set_error(YGG_ERR_INVALID_ARGUMENT, "capacity %d < %d level nodes", capacity, lv.num_nodes);
+  for (int j = 0; j < lv.num_nodes; j++) {
+    const bool scanned = tab[lv.first_node + j].candidate != 0;
+    for (int fl = 0; fl < c.f_scan; fl++) {
+      const size_t i = static_cast<size_t>(j) * c.f_scan + fl;
+      tried[i] = scanned ? flags[i] : 0;
+    }
+  }
   return YGG_OK;
 }
 

@@ -370,6 +370,9 @@ struct ScanParams {
   // counts keep deciding min_examples
   int weighted;
   double w_inv;
+  // candidate feature sampling (DESIGN.md §23): [level nodes][f_count] 1 when the scan tried at least one boundary of the
+  // (node, feature) pair (the reference's status is then not kInvalidAttribute); null when sampling is off
+  uint8_t* tried;
 };
 
 __device__ __forceinline__ double l1_threshold_d(double v, double l1) {
@@ -402,14 +405,23 @@ __device__ __forceinline__ Scan3 block_inclusive_scan(Scan3 v, Scan3* s_warp /*[
   return v;
 }
 
+// Whether ScanSplits scores the boundary at all (splitter_scanner.h:1007-1041, where it sets tried_one_split): `in_range`
+// (not the last bucket) and at least min_num_obs rows on each side.  The label accumulators' IsValidSplit is always true
+// (splitter_accumulator.h:917-920, :1521-1524), so a side without weight still counts as tried.  A feature none of whose
+// boundaries passes is kInvalidAttribute for its node.
+__device__ __forceinline__ bool boundary_tried(const ScanParams& p, const Scan3& tot, const Scan3& inc, bool in_range) {
+  const long long n_neg = inc.c, n_pos = tot.c - inc.c;
+  return in_range && (n_pos >= p.min_num_obs) && (n_neg >= p.min_num_obs);
+}
+
 // Score of the numerical boundary whose negative side holds the sums `inc` of a node with the sums `tot` (bucket
 // interpolation aside, ScanSplits' per-boundary step, splitter_scanner.h:931-1101) in *score_out; false when it is not a
-// valid split: `in_range` false (the last bucket), a side below min_num_obs rows (or without weight), or a score not above
-// the minimum.  Shared by the byte scan (scan_node) and the wide-column scan (k_scan_wide, ygg_wide.cuh).
+// valid split: not boundary_tried, a side without weight, or a score not above the minimum.  Shared by the byte scan (scan_node) and the
+// wide-column scan (k_scan_wide, ygg_wide.cuh).
 __device__ __forceinline__ bool boundary_score(const ScanParams& p, const Scan3& tot, const Scan3& inc, bool in_range,
                                                double ginv, double hinv, double* score_out) {
   const long long n_neg = inc.c, n_pos = tot.c - inc.c;
-  bool valid = in_range && (n_pos >= p.min_num_obs) && (n_neg >= p.min_num_obs);
+  bool valid = boundary_tried(p, tot, inc, in_range);
   double score = 0.0;
   double min_score = 0.0;
   if (!p.use_hessian) {
@@ -471,8 +483,9 @@ __device__ __forceinline__ bool boundary_score(const ScanParams& p, const Scan3&
 }
 
 // Scans one node's 256-bin histogram held one bin per thread; thread 0 writes the Candidate.
+// tried_out (or null): the node's validity flag for candidate feature sampling (ScanParams.tried).
 __device__ void scan_node(const ScanParams& p, const NodeRec& node, int f_global, long long cnt,
-                          long long sq /*unbiased quantised sum*/, long long hq, Candidate* out) {
+                          long long sq /*unbiased quantised sum*/, long long hq, Candidate* out, uint8_t* tried_out) {
   __shared__ Scan3 s_warp[8];
   __shared__ double s_best_score[8];
   __shared__ int s_best_b[8];
@@ -486,6 +499,10 @@ __device__ void scan_node(const ScanParams& p, const NodeRec& node, int f_global
   const long long n_pos = tot.c - inc.c;
   double score;
   const bool valid = boundary_score(p, tot, inc, b <= B - 2, ginv, hinv, &score);
+  if (tried_out != nullptr) {
+    const int tried = __syncthreads_or(boundary_tried(p, tot, inc, b <= B - 2));
+    if (b == 0) *tried_out = tried ? 1 : 0;
+  }
   // arg-max with the lowest bin on ties (sequential strict '>' keeps the first maximum).
   double bs = valid ? score : -1.0;
   int bb = valid ? b : 0x7fffffff;
@@ -562,7 +579,7 @@ __device__ __forceinline__ double category_key(const ScanParams& p, long long cn
 // form the positive set (splitter_accumulator.h:391-411).  Equal keys are ordered by category
 // index (the reference's std::sort leaves that order unspecified; DESIGN.md §6).
 __device__ void scan_node_categorical(const ScanParams& p, const NodeRec& node, int f_global, long long cnt,
-                                      long long sq, long long hq, Candidate* out, uint32_t* mask_out) {
+                                      long long sq, long long hq, Candidate* out, uint32_t* mask_out, uint8_t* tried_out) {
   __shared__ double s_key[kMaxBins];
   __shared__ int s_idx[kMaxBins];
   __shared__ long long s_cnt[kMaxBins], s_sq[kMaxBins], s_hq[kMaxBins];
@@ -602,6 +619,10 @@ __device__ void scan_node_categorical(const ScanParams& p, const NodeRec& node, 
   sp.l2 = p.l2_categorical;
   double score;
   const bool valid = boundary_score(sp, tot, inc, b <= B - 2, ginv, hinv, &score);
+  if (tried_out != nullptr) {
+    const int tried = __syncthreads_or(boundary_tried(sp, tot, inc, b <= B - 2));
+    if (b == 0) *tried_out = tried ? 1 : 0;
+  }
   double bs = valid ? score : -1.0;
   int bb = valid ? b : 0x7fffffff;
 #pragma unroll
@@ -659,12 +680,13 @@ __global__ void __launch_bounds__(256) k_scan(ScanParams p) {
   const bool categorical = p.feature_type[f_global] == 1;
   if (direct.candidate) {
     const size_t ci = static_cast<size_t>(fam.direct - lv.first_node) * p.f_count + fl;
+    uint8_t* tried = p.tried != nullptr ? p.tried + ci : nullptr;
     if (categorical)
       scan_node_categorical(p, direct, f_global, cnt_d, static_cast<long long>(sum_d) - cnt_d * static_cast<long long>(kQBias),
-                            static_cast<long long>(hs_d), &p.cand[ci], p.cand_mask + ci * 8);
+                            static_cast<long long>(hs_d), &p.cand[ci], p.cand_mask + ci * 8, tried);
     else
       scan_node(p, direct, f_global, cnt_d, static_cast<long long>(sum_d) - cnt_d * static_cast<long long>(kQBias),
-                static_cast<long long>(hs_d), &p.cand[ci]);
+                static_cast<long long>(hs_d), &p.cand[ci], tried);
   }
   if (fam.derived >= 0) {
     const NodeRec derived = p.nodes[fam.derived];
@@ -682,12 +704,13 @@ __global__ void __launch_bounds__(256) k_scan(ScanParams p) {
         if (HESS && p.has_h) p.hist_hsum[ox] = hs_x;
       }
       const size_t cx = static_cast<size_t>(fam.derived - lv.first_node) * p.f_count + fl;
+      uint8_t* tried = p.tried != nullptr ? p.tried + cx : nullptr;
       if (categorical)
         scan_node_categorical(p, derived, f_global, cnt_x, static_cast<long long>(sum_x) - cnt_x * static_cast<long long>(kQBias),
-                              static_cast<long long>(hs_x), &p.cand[cx], p.cand_mask + cx * 8);
+                              static_cast<long long>(hs_x), &p.cand[cx], p.cand_mask + cx * 8, tried);
       else
         scan_node(p, derived, f_global, cnt_x, static_cast<long long>(sum_x) - cnt_x * static_cast<long long>(kQBias),
-                  static_cast<long long>(hs_x), &p.cand[cx]);
+                  static_cast<long long>(hs_x), &p.cand[cx], tried);
     }
   }
 }
@@ -747,6 +770,31 @@ __device__ __forceinline__ float candidate_thr_value(const SelectParams& p, int 
   if (p.wide_thr_value != nullptr && ((p.wide_of != nullptr && p.wide_of[fg] >= 0) || p.feature_type[fg] == 2))
     return p.wide_thr_value[static_cast<size_t>(j) * p.f_count + fl];
   return p.bucket_values != nullptr ? thr_value_of(thr, p.bucket_values + static_cast<size_t>(fg) * kMaxBins) : __builtin_nanf("");
+}
+
+// This shard's best split of level node j: local feature best_f (0x7fffffff: none) with its candidate, for
+// k_select_sampled.  k_select_local writes the same record inline (a call there compiles to a different schedule).
+__device__ __forceinline__ void write_shard_best(const SelectParams& p, int j, int best_f, float best_score, const Candidate& best_c) {
+  ShardBest out{};
+  out.feature = -1;
+  if (best_f != 0x7fffffff) {
+    const int fg = p.f_begin + best_f;
+    out.score = best_score; out.feature = fg; out.thr = best_c.thr; out.n_pos = best_c.n_pos;
+    out.cond_type = p.feature_type[fg];
+    if (out.cond_type == 1) {
+      const uint32_t* m = p.cand_mask + (static_cast<size_t>(j) * p.f_count + best_f) * 8;
+      const int na = p.na_bin[fg];
+#pragma unroll
+      for (int i = 0; i < 8; i++) out.mask[i] = m[i];
+      out.na_value = (m[na >> 5] >> (na & 31)) & 1u;  // NA replacement in the positive set
+      const int wi = wide_cat_index(p, fg, 1);
+      if (wi >= 0) {   // (its byte mask is the filler's: empty)
+        const int wna = p.wide_na_bin[wi];
+        out.na_value = (wide_set_of(p, j, wi)[wna >> 5] >> (wna & 31)) & 1u;
+      }
+    }
+  }
+  p.shard_best[static_cast<size_t>(p.rank) * p.max_level_nodes + j] = out;
 }
 
 __global__ void __launch_bounds__(256) k_select_local(SelectParams p) {
@@ -861,6 +909,122 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int* s_warp /*[32]*/,
   __syncthreads();
   *total = tot;
   return off + incl - v;
+}
+
+// Candidate feature sampling (DESIGN.md §23): the selection of k_select_local restricted, per node, to the first
+// `k_valid` features of the node's candidate order that the scan tried (ScanParams.tried), all of them when fewer are.
+// The order is ascending (candidate_key(seed, tree, node, f), f) — the reference's per-node shuffle
+// (GetCandidateAttributes, training.cc:4246-4306) made a function of the node — and the first maximum in that order
+// wins (strict '>': lowest key among equal float scores).
+struct SampleParams {
+  const uint8_t* tried;   // [level nodes][f_count]
+  int k_valid;            // k (concurrent manager) or k + 1 (single-thread manager)
+  uint32_t seed;
+  int32_t tree;
+};
+
+// 96-bit candidate-order position (key, f) of a feature, split into 12 radix digits of 8 bits, most significant first.
+__device__ __forceinline__ uint32_t order_digit(uint64_t key, uint32_t f, int d) {
+  return d < 8 ? static_cast<uint32_t>(key >> (56 - 8 * d)) & 0xFFu : (f >> (24 - 8 * (d - 8))) & 0xFFu;
+}
+
+// One CTA of 256 threads per node of the level.  A block-wide radix select finds the (key, f) of the k_valid-th tried
+// feature in 12 passes over the node's features (one 256-bin histogram of the next digit per pass), then an ordered
+// arg-max runs over the features at or before it.
+__global__ void __launch_bounds__(256) k_select_sampled(SelectParams p, SampleParams s) {
+  __shared__ int s_hist[256];
+  __shared__ int s_warp[32];
+  __shared__ uint64_t s_key;
+  __shared__ uint32_t s_f;
+  __shared__ int s_rank;
+  __shared__ float s_score[8];
+  __shared__ uint64_t s_bkey[8];
+  __shared__ int s_bf[8];
+  const LevelDesc lv = p.levels[p.level];
+  const int j = blockIdx.x;
+  if (j >= lv.num_nodes) return;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  const int node = lv.first_node + j;
+  const bool cand_node = p.nodes[node].candidate != 0;
+  const uint8_t* tried = s.tried + static_cast<size_t>(j) * p.f_count;
+  // tried features of the node
+  int mine = 0;
+  if (cand_node)
+    for (int fl = tid; fl < p.f_count; fl += blockDim.x) mine += tried[fl];
+  int n_valid;
+  block_exclusive_scan(mine, s_warp, &n_valid);
+  // cutoff = the (key, f) of the k_valid-th tried feature in the candidate order; every feature when there are no more
+  uint64_t cut_key = ~0ull;
+  uint32_t cut_f = 0xFFFFFFFFu;
+  if (n_valid > s.k_valid) {
+    if (tid == 0) { s_key = 0ull; s_f = 0u; s_rank = s.k_valid - 1; }
+    for (int d = 0; d < 12; d++) {
+      s_hist[tid] = 0;
+      __syncthreads();
+      const uint64_t pk = s_key;
+      const uint32_t pf = s_f;
+      for (int fl = tid; fl < p.f_count; fl += blockDim.x) {
+        if (!tried[fl]) continue;
+        const uint32_t fg = static_cast<uint32_t>(p.f_begin + fl);
+        const uint64_t key = candidate_key(s.seed, s.tree, node, fg);
+        // the digits above d must equal the selected prefix
+        bool match = true;
+        for (int e = 0; e < d; e++) match = match && order_digit(key, fg, e) == order_digit(pk, pf, e);
+        if (match) atomicAdd(&s_hist[order_digit(key, fg, d)], 1);
+      }
+      __syncthreads();
+      const int c = s_hist[tid];
+      int total;
+      const int below = block_exclusive_scan(c, s_warp, &total);
+      const int rank = s_rank;
+      __syncthreads();
+      if (below <= rank && rank < below + c) {   // exactly one digit holds the rank
+        if (d < 8) s_key = pk | (static_cast<uint64_t>(tid) << (56 - 8 * d));
+        else s_f = pf | (static_cast<uint32_t>(tid) << (24 - 8 * (d - 8)));
+        s_rank = rank - below;
+      }
+      __syncthreads();
+    }
+    cut_key = s_key;
+    cut_f = s_f;
+  }
+  // ordered arg-max over the found candidates at or before the cutoff
+  float best_score = 0.f;   // NodeCondition.split_score default: a split needs score > 0
+  uint64_t best_key = ~0ull;
+  int best_f = 0x7fffffff;
+  if (cand_node) {
+    for (int fl = tid; fl < p.f_count; fl += blockDim.x) {
+      const Candidate c = p.cand[static_cast<size_t>(j) * p.f_count + fl];
+      if (!c.found) continue;
+      const uint32_t fg = static_cast<uint32_t>(p.f_begin + fl);
+      const uint64_t key = candidate_key(s.seed, s.tree, node, fg);
+      if (key > cut_key || (key == cut_key && fg > cut_f)) continue;
+      if (c.score > best_score || (c.score == best_score && best_f != 0x7fffffff && key < best_key)) {
+        best_score = c.score; best_key = key; best_f = fl;
+      }
+    }
+  }
+  // (keys are distinct per (key, f) order: equal keys fall back to the feature index)
+  auto better = [](float as, uint64_t ak, int af, float bs, uint64_t bk, int bf) {
+    if (af == 0x7fffffff) return false;
+    if (bf == 0x7fffffff) return true;
+    return as > bs || (as == bs && (ak < bk || (ak == bk && af < bf)));
+  };
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float os = __shfl_xor_sync(0xffffffffu, best_score, o);
+    const uint64_t ok = __shfl_xor_sync(0xffffffffu, best_key, o);
+    const int of = __shfl_xor_sync(0xffffffffu, best_f, o);
+    if (better(os, ok, of, best_score, best_key, best_f)) { best_score = os; best_key = ok; best_f = of; }
+  }
+  if (lane == 0) { s_score[w] = best_score; s_bkey[w] = best_key; s_bf[w] = best_f; }
+  __syncthreads();
+  if (tid == 0) {
+    for (int i = 1; i < static_cast<int>(blockDim.x >> 5); i++)
+      if (better(s_score[i], s_bkey[i], s_bf[i], best_score, best_key, best_f)) { best_score = s_score[i]; best_key = s_bkey[i]; best_f = s_bf[i]; }
+    const Candidate best_c = best_f != 0x7fffffff ? p.cand[static_cast<size_t>(j) * p.f_count + best_f] : Candidate{0.f, 0, 0, 0};
+    write_shard_best(p, j, best_f, best_score, best_c);
+  }
 }
 
 __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* a) {

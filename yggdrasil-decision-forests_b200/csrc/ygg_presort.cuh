@@ -104,9 +104,11 @@ __device__ __forceinline__ Scan3 presort_range(const PresortParams& p, int64_t l
   return Scan3{c, static_cast<long long>(s) - c * static_cast<long long>(kQBias), static_cast<long long>(h)};
 }
 
-// Score of the boundary after list entry i (false: no valid boundary there).  *slot = the (level node, column) pair.
+// Score of the boundary after list entry i (false: no valid boundary there).  *slot = the (level node, column) pair;
+// *tried = boundary_tried there (false: no boundary between two different values).
 template <bool HESS>
-__device__ __forceinline__ bool presort_boundary(const PresortParams& p, int64_t i, int64_t m, double* score, int64_t* slot) {
+__device__ __forceinline__ bool presort_boundary(const PresortParams& p, int64_t i, int64_t m, double* score, int64_t* slot,
+                                                 bool* tried) {
   const int64_t col = (i / p.n) * p.n;
   if (i - col >= m) return false;
   const int node = p.node_of_row[p.row[i]];
@@ -117,6 +119,7 @@ __device__ __forceinline__ bool presort_boundary(const PresortParams& p, int64_t
   const double ginv = static_cast<double>(p.s.st->g_pow2) / static_cast<double>(1u << (kQBits - 1));
   const double hinv = static_cast<double>(p.s.st->h_pow2) / static_cast<double>(1u << kQBits);
   *slot = static_cast<int64_t>(node - p.s.levels[p.level].first_node) * p.P + i / p.n;
+  *tried = boundary_tried(p.s, tot, inc, true);
   return boundary_score(p.s, tot, inc, true, ginv, hinv, score);
 }
 
@@ -133,7 +136,11 @@ __global__ void __launch_bounds__(256) k_presort_scan(PresortParams p) {
     const int64_t i = w0 + lane;
     double score = 0.0;
     int64_t slot = -1;
-    const bool valid = i < total && presort_boundary<HESS>(p, i, m, &score, &slot);
+    bool tried = false;
+    const bool valid = i < total && presort_boundary<HESS>(p, i, m, &score, &slot, &tried);
+    // (k_scan left 0 for the pair: its filler column has one bucket)
+    if (MAX_PASS && tried && p.s.tried != nullptr)
+      p.s.tried[static_cast<size_t>(slot / p.P) * p.s.f_count + (p.num_feature[slot % p.P] - p.s.f_begin)] = 1;
     if (!valid) slot = -1;
     unsigned long long key = 0ull;   // MAX_PASS: the score's bits; else the candidate index (or ~0)
     if (MAX_PASS) key = valid ? static_cast<unsigned long long>(__double_as_longlong(score)) : 0ull;

@@ -123,6 +123,7 @@ __device__ void scan_wide_node(const WideScanParams& p, int node, int fl, int B,
   int bb = 0x7fffffff;
   long long bnpos = 0;
   Scan3 carry{0, 0, 0};
+  bool tried = false;
   for (int t0 = 0; t0 < B; t0 += blockDim.x) {
     const int b = t0 + tid;
     const Scan3 v = b < B ? wide_bucket<HESS>(p, d, x, derived, b) : Scan3{0, 0, 0};
@@ -132,6 +133,11 @@ __device__ void scan_wide_node(const WideScanParams& p, int node, int fl, int B,
     carry.c += tile.c; carry.s += tile.s; carry.h += tile.h;
     double score;
     if (boundary_score(p.s, tot, inc, b <= B - 2, ginv, hinv, &score) && score > bs) { bs = score; bb = b; bnpos = tot.c - inc.c; }
+    if (p.s.tried != nullptr) tried = tried || boundary_tried(p.s, tot, inc, b <= B - 2);
+  }
+  if (p.s.tried != nullptr) {
+    const int any = __syncthreads_or(tried);
+    if (tid == 0) p.s.tried[static_cast<size_t>(node - lv.first_node) * p.s.f_count + fl] = any ? 1 : 0;
   }
   const int my_b = bb;
 #pragma unroll
@@ -283,6 +289,7 @@ __device__ void scan_wide_cat_node(const WideScanParams& p, int node, int fl, in
   int bb = 0x7fffffff;
   long long bnpos = 0;
   Scan3 carry{0, 0, 0};
+  bool tried = false;
   for (int t0 = 0; t0 < B; t0 += blockDim.x) {
     const int pos = t0 + tid;
     const Scan3 v = pos < B ? wide_bucket<HESS>(p, d, x, derived, idx[pos]) : Scan3{0, 0, 0};
@@ -292,6 +299,11 @@ __device__ void scan_wide_cat_node(const WideScanParams& p, int node, int fl, in
     carry.c += tile.c; carry.s += tile.s; carry.h += tile.h;
     double score;
     if (boundary_score(sp, tot, inc, pos <= B - 2, ginv, hinv, &score) && score > bs) { bs = score; bb = pos; bnpos = tot.c - inc.c; }
+    if (p.s.tried != nullptr) tried = tried || boundary_tried(sp, tot, inc, pos <= B - 2);
+  }
+  if (p.s.tried != nullptr) {
+    const int any = __syncthreads_or(tried);
+    if (tid == 0) p.s.tried[static_cast<size_t>(node - lv.first_node) * p.s.f_count + fl] = any ? 1 : 0;
   }
   const int my_b = bb;
 #pragma unroll

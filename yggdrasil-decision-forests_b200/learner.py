@@ -66,6 +66,8 @@ class GradientBoostedTreesLearner:
                  goss_beta: float = 0.1,
                  growing_strategy: str = "LOCAL",
                  max_num_nodes: int = 31,
+                 num_candidate_attributes: int = -1,
+                 num_candidate_attributes_ratio: Optional[float] = None,
                  forest_extraction: str = "MART",
                  random_seed: int = 123456,
                  num_threads: Optional[int] = None,
@@ -142,6 +144,25 @@ class GradientBoostedTreesLearner:
         if growing_strategy not in ("LOCAL", "BEST_FIRST_GLOBAL"):
             raise ValueError(f"unknown growing_strategy {growing_strategy!r}")
         self.growing_strategy = growing_strategy
+        # Candidate feature sampling (DecisionTreeTrainingConfig.num_candidate_attributes / _ratio): each node is split on
+        # the best of k features taken in a per-node random order (ygg_gbt_set_candidate_sampling, DESIGN.md §23).
+        # -1 / None: every feature; 0 or a ratio of 0: the task's default (sqrt(F) classification, F/3 regression).
+        if isinstance(num_candidate_attributes, bool) or not isinstance(num_candidate_attributes, (int, np.integer)):
+            raise TypeError("num_candidate_attributes must be an integer")
+        if int(num_candidate_attributes) < -1:
+            raise ValueError("num_candidate_attributes must be >= -1 (-1: every feature, 0: the task's default)")
+        if num_candidate_attributes_ratio is not None:
+            if isinstance(num_candidate_attributes_ratio, bool) or \
+                    not isinstance(num_candidate_attributes_ratio, (int, float, np.integer, np.floating)):
+                raise TypeError("num_candidate_attributes_ratio must be a number or None")
+            if not 0.0 <= float(num_candidate_attributes_ratio) <= 1.0:
+                raise ValueError("num_candidate_attributes_ratio must be in [0, 1]")
+            if int(num_candidate_attributes) != -1:
+                raise ValueError("Only one of the following hyperparameters can be set: num_candidate_attributes, "
+                                 "num_candidate_attributes_ratio")
+        self.num_candidate_attributes = int(num_candidate_attributes)
+        self.num_candidate_attributes_ratio = (None if num_candidate_attributes_ratio is None
+                                               else float(num_candidate_attributes_ratio))
         if forest_extraction != "MART":
             raise NotImplementedError("only forest_extraction=MART is implemented")
         if task == Task.CLASSIFICATION:
@@ -182,6 +203,7 @@ class GradientBoostedTreesLearner:
         self.cfg.max_num_nodes = int(max_num_nodes)
         # (the shuffle replay follows the depth-first order of the local growth)
         self.cfg.candidate_shuffle = 0 if self.cfg.growing_strategy else _TIE_BREAK[tie_break]
+        self._candidate_shuffle = self.cfg.candidate_shuffle
         self.cfg.split_jobs_draw_seeds = int(self.num_threads > 1)   # FindBestConditionConcurrentManager, training.cc:1658
 
     # -- dataspec + device dataset -----------------------------------------------------------------
@@ -365,8 +387,14 @@ class GradientBoostedTreesLearner:
                     valid_labels, labels = labels[~in_training], labels[in_training]
                     if weights is not None:
                         valid_weights, weights = weights[~in_training], weights[in_training]
+            # with candidate sampling the per-node keys order the candidates: no tie-break replay (as best-first growth)
+            k = _capi.num_candidate_attributes(train_ds.n_features, self.cfg.loss, self.num_candidate_attributes,
+                                               self.num_candidate_attributes_ratio)
+            self.cfg.candidate_shuffle = 0 if k < train_ds.n_features else self._candidate_shuffle
             gbt = _capi.Gbt(train_ds, self.cfg)
             try:
+                if k < train_ds.n_features:
+                    gbt.set_candidate_sampling(self.num_candidate_attributes, self.num_candidate_attributes_ratio)
                 if weights is not None:
                     gbt.set_weights(weights)     # before the labels: the initial predictions are weighted
                 gbt.set_labels(labels)
@@ -390,8 +418,9 @@ class GradientBoostedTreesLearner:
             for d in (train_ds, valid_ds, full):
                 if d is not None:
                     d.close()
-        model = GradientBoostedTreesModel(spec, trees, init, self.loss, logs,
-                                          config={k: getattr(self.cfg, k) for k, _ in self.cfg._fields_},
-                                          category_sets=category_sets)
+        config = {k: getattr(self.cfg, k) for k, _ in self.cfg._fields_}
+        config["num_candidate_attributes"] = self.num_candidate_attributes
+        config["num_candidate_attributes_ratio"] = self.num_candidate_attributes_ratio
+        model = GradientBoostedTreesModel(spec, trees, init, self.loss, logs, config=config, category_sets=category_sets)
         model.validation_loss, model.early_stopping_triggered = final
         return model
