@@ -20,6 +20,7 @@ import pytest
 
 import ydf_b200
 from tests import scan_ref as S
+from tests.boost_ref import route
 from tests.util import quantize_q24, quantize_second
 
 pytestmark = pytest.mark.gpu
@@ -29,33 +30,6 @@ def byte_cols(bins, num_bins, ftypes, bucket_values=None):
     """Column descriptions of byte columns: (kind, codes, buckets, bucket values or None)."""
     bucket_values = bucket_values or {}
     return [("cat" if ftypes[f] == 1 else "num", bins[f], int(num_bins[f]), bucket_values.get(f)) for f in range(len(bins))]
-
-
-def route(tree, cols, sets=None):
-    """{pre-order node: row indices} of every node: byte and wide codes against threshold_bin or the category mask /
-    wide positive set (`sets`, Gbt.get_category_sets), presorted values ('pre': the stored values) >= threshold_value."""
-    out = {}
-    sets = sets or {}
-
-    def walk(i, rows):
-        out[i] = rows
-        nd = tree[i]
-        if nd["feature"] < 0:
-            return
-        kind, codes, _, _ = cols[nd["feature"]]
-        if kind == "pre":
-            go = codes[rows] >= nd["threshold_value"]
-        elif nd["condition_type"] == 1:
-            b = codes[rows].astype(np.int64)
-            words = sets[i] if kind == "wide_cat" else nd["cat_mask"]
-            go = ((words[b >> 5] >> (b & 31).astype(np.uint32)) & 1) != 0
-        else:
-            go = codes[rows].astype(np.int64) >= nd["threshold_bin"]
-        walk(int(nd["neg_child"]), rows[~go])
-        walk(int(nd["pos_child"]), rows[go])
-
-    walk(0, np.arange(len(cols[0][1])))
-    return out
 
 
 def ulp32(x):
