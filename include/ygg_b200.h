@@ -269,7 +269,8 @@ int ygg_gbt_set_validation_f32(ygg_gbt* h, const ygg_dataset* valid, const float
 /* Weights of the validation rows (the hold-out is cut from the weighted dataset, gradient_boosted_trees.cc:1262-1280):
  * validation loss and accuracy become weighted.  After ygg_gbt_set_validation_*, before training. */
 int ygg_gbt_set_validation_weights_f32(ygg_gbt* h, const float* weights, int64_t n);
-/* Validation loss / secondary metric after iteration `iter` (TrainingLogs.Entry.validation_loss). */
+/* Validation loss / secondary metric after iteration `iter` (TrainingLogs.Entry.validation_loss); `iter` below
+ * ygg_gbt_num_iterations (early stopping trains whole batches: the iterations past the stop have no entry). */
 int ygg_gbt_validation_loss(ygg_gbt* h, int32_t iter, float* loss, float* secondary);
 /* Iterations with log entries; > ygg_gbt_num_trees when the model was truncated. */
 int32_t ygg_gbt_num_iterations(const ygg_gbt* h);
@@ -405,7 +406,7 @@ int ygg_gbt_get_tree(ygg_gbt* h, int32_t iter, ygg_node* out, int32_t capacity, 
 int ygg_gbt_get_category_set(ygg_gbt* h, int32_t iter, int32_t node, uint32_t* words, int32_t capacity, int32_t* n_words);
 /* Training loss / secondary metric after iteration `iter` (loss->Loss,
  * gradient_boosted_trees.cc:1575-1580): binomial => (2x mean log-loss, accuracy);
- * squared error => (rmse, rmse). */
+ * squared error => (rmse, rmse).  `iter` below ygg_gbt_num_iterations. */
 int ygg_gbt_train_loss(ygg_gbt* h, int32_t iter, float* loss, float* secondary);
 /* Current raw predictions (logits / regression values), N floats to host. */
 int ygg_gbt_get_predictions(ygg_gbt* h, float* out, int64_t n);

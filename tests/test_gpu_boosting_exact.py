@@ -97,9 +97,14 @@ class Table:
 # ---------------------------------------------------------------------------------------------------------------------
 # the driver
 
-def check_run(gbt, cfg, table, labels, vlabels=None, weights=None, iters=3, step=False):
+def check_run(gbt, cfg, table, labels, vlabels=None, weights=None, iters=3, step=False, vweights=None, on_tree=None,
+              trained=False, logged=None, kept_trees=None):
     """Trains `iters` iterations (one train() call, or step() + get_predictions() per iteration) and checks every stage
     against the reference.  labels: binomial {1, 2}, multinomial 1..K, squared error floats.
+    vweights: the held-out rows' weights.  on_tree(t, rows): called after each tree's checks with the per-row quantities
+    it was trained on (dict g, h, g_alt, h_alt, sel, w); with step=True before the next step(), so that the tree's
+    candidate capture is still the live one.  trained=True: the caller already trained `iters` iterations (train() with
+    early stopping), of which `logged` have losses and whose model keeps the first `kept_trees` trees.
     -> (number of nodes checked, the reference's (P, g2w power of two or None) of every tree)."""
     n = table.n
     loss = int(cfg.loss)
@@ -109,20 +114,18 @@ def check_run(gbt, cfg, table, labels, vlabels=None, weights=None, iters=3, step
     sub = cfg.subsample < 1.0
     weighted = weights is not None or goss
     labels = np.asarray(labels)
+    logged = iters if logged is None else logged
+    kept_trees = iters * K if kept_trees is None else kept_trees
     stepped = []
-    if step:
-        for _ in range(iters):
-            gbt.step()
-            stepped.append(gbt.get_predictions().copy())
-    else:
+    if not step and not trained:
         gbt.train(iters)
     init = F32(gbt.initial_prediction())
-    trees = [gbt.get_tree(t) for t in range(iters * K)]
     wide_cat = any(c[0] == "wide_cat" for c in table.cols)
-    sets = [gbt.get_category_sets(t, trees[t]) if wide_cat else {} for t in range(iters * K)]
     pred = np.full((K, n), init, F32)
     vpred = np.full((K, table.n_valid), init, F32) if vlabels is not None else None
+    kept = (pred.copy(), None if vpred is None else vpred.copy()) if kept_trees == 0 else None
     rng = O.Rng(int(cfg.random_seed))
+    rng.discard(int(cfg.rng_words_consumed))   # the row draws share the learner's stream, after those words
     if weights is not None:
         w_pow2 = R.pow2_cover(np.max(weights))
     elif goss:
@@ -134,6 +137,9 @@ def check_run(gbt, cfg, table, labels, vlabels=None, weights=None, iters=3, step
         w_pow2 = None
     errs, checked, scales = [], 0, []
     for it in range(iters):
+        if step:
+            gbt.step()
+            stepped.append(gbt.get_predictions().copy())
         # per-row gradients from the predictions before the iteration
         if loss == 2:
             cls = labels - 1
@@ -154,7 +160,8 @@ def check_run(gbt, cfg, table, labels, vlabels=None, weights=None, iters=3, step
             sel = R.subsample_mask(rng, n, cfg.subsample)
         for k in range(K):
             t = it * K + k
-            tree = trees[t]
+            tree = gbt.get_tree(t)
+            sets = gbt.get_category_sets(t, tree) if wide_cat else {}
             if weighted:
                 gk, hk, g2w = R.weigh(g[k], h[k], w, unit_hessian=not logit)
                 gk_alt, hk_alt, g2w_alt = R.weigh(g_alt[k], h_alt[k], w, unit_hessian=not logit)
@@ -166,32 +173,42 @@ def check_run(gbt, cfg, table, labels, vlabels=None, weights=None, iters=3, step
             rows = R.Rows(gk, hk if has_h else None, sel, P, h_pow2, g_alt=gk_alt, h_alt=hk_alt if has_h else None,
                           w=w if weighted else None, w_pow2=w_pow2, g2w=g2w, g2w_alt=g2w_alt)
             scales.append((P, rows.g2pow2 if weighted else None))
-            rows_of = R.route(tree, table.cols, sets[t])
+            rows_of = R.route(tree, table.cols, sets)
             errs += R.check_tree(tree, rows_of, rows, cfg, logit, where=f"tree {t}")
             checked += len(tree)
             leaf = R.leaf_of_rows(tree, rows_of, n)
             pred[k] = (pred[k] + tree["leaf_value"][leaf]).astype(F32)
             if vpred is not None:
-                vrows = R.route(tree, table.vcols, sets[t])
+                vrows = R.route(tree, table.vcols, sets)
                 vpred[k] = (vpred[k] + tree["leaf_value"][R.leaf_of_rows(tree, vrows, table.n_valid)]).astype(F32)
+            if t + 1 == kept_trees:
+                kept = (pred.copy(), None if vpred is None else vpred.copy())
+            if on_tree is not None:
+                on_tree(t, dict(g=gk, h=hk if has_h else None, g_alt=gk_alt, h_alt=hk_alt if has_h else None, sel=sel,
+                                w=w if weighted else None, tree=tree))
         if step:
             got = stepped[it] if K == 1 else stepped[it].T
             if not np.array_equal(got.reshape(K, n), pred):
                 errs.append(f"iteration {it}: get_predictions after step() differ in {int((got.reshape(K, n) != pred).sum())} rows")
+        if it >= logged:
+            continue
         errs += check_losses(gbt.train_loss(it), loss, pred, labels, weights, w_pow2 if weights is not None else None,
                              f"train loss {it}")
         if vpred is not None:
-            errs += check_losses(gbt.validation_loss(it), loss, vpred, np.asarray(vlabels), None, None, f"validation loss {it}")
+            vw_pow2 = R.pow2_cover(np.max(vweights)) if vweights is not None else None
+            errs += check_losses(gbt.validation_loss(it), loss, vpred, np.asarray(vlabels), vweights, vw_pow2,
+                                 f"validation loss {it}")
     got = gbt.get_predictions()
     got = got[None] if K == 1 else got.T
     if not np.array_equal(got, pred):
         errs.append(f"get_predictions differ in {int((got != pred).sum())} values")
+    # predict() evaluates the model: the first kept_trees trees
     p = gbt.predict(table.ds)
-    if not np.array_equal(p[None] if K == 1 else p.T, pred):
+    if not np.array_equal(p[None] if K == 1 else p.T, kept[0]):
         errs.append("predict(training table) differs from the leaf sums")
     if vpred is not None:
         p = gbt.predict(table.vds)
-        if not np.array_equal(p[None] if K == 1 else p.T, vpred):
+        if not np.array_equal(p[None] if K == 1 else p.T, kept[1]):
             errs.append("predict(held-out table) differs from the leaf sums")
     assert not errs, f"{len(errs)} mismatches:\n" + "\n".join(errs[:30])
     return checked, scales

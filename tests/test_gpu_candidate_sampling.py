@@ -23,12 +23,17 @@ def k_valid(cfg, F, num=-1, ratio=None):
     return k if cfg.split_jobs_draw_seeds else k + 1
 
 
-def check_levels(gbt, cfg, tree, tree_index, kv, cols=None, g=None, h=None):
+def check_levels(gbt, cfg, tree, tree_index, kv, cols=None, g=None, h=None, sel=None, w=None, trained_tree=False):
     """Selection of every captured level node against the restatement; with `cols` (route's column descriptions) also
-    every validity flag against the rows' tried predicate (the tree is then a train_tree_on_gradients one).
+    every validity flag against the tried predicate of the node's rows: all rows, or those of `sel` (subsample / GOSS),
+    the gradients `g` (w*g with example weights `w`) and hessians `h` of the tree.  The tree is the last
+    train_tree_on_gradients one, or with trained_tree=True tree `tree_index` of the training.
     -> (nodes checked, flags checked, invalid flags seen)."""
-    sets = gbt.get_category_sets(-1, tree) if cols and any(c[0] == "wide_cat" for c in cols) else {}
+    wide_cat = cols and any(c[0] == "wide_cat" for c in cols)
+    sets = gbt.get_category_sets(tree_index if trained_tree else -1, tree) if wide_cat else {}
     rows_of = route(tree, cols, sets) if cols else None
+    if rows_of is not None and sel is not None:
+        rows_of = {i: r[sel[r]] for i, r in rows_of.items()}
     min_obs = cfg.min_examples if cfg.in_split_min_examples_check else 1
     nodes = flags = invalid = 0
     for level in range(cfg.max_depth - 1):
@@ -56,13 +61,17 @@ def check_levels(gbt, cfg, tree, tree_index, kv, cols=None, g=None, h=None):
                 elif kind in ("cat", "wide_cat") and min_obs > 1:
                     P = cap["P"]
                     q = quantize_q24(g, P)
-                    if h is not None:
+                    w_inv = None
+                    if w is not None:
+                        w_inv = cap["w_pow2"] / 2.0 ** 24
+                        hq, hinv = quantize_second(w, cap["w_pow2"]), w_inv
+                    elif h is not None:
                         hq, hinv = quantize_second(h, cap["h_pow2"]), cap["h_pow2"] / 2.0 ** 24
                     else:
                         hq, hinv = np.full(len(g), 2 ** 24, np.int64), cap["h_pow2"] / 2.0 ** 24
                     c, s, hs = S.bucket_sums(codes, rows, q, hq, B)
                     keys = S.category_keys(c, s, hs, bool(cfg.use_hessian_gain), P / 2.0 ** 23, hinv,
-                                           cfg.l1_regularization, cfg.l2_regularization_categorical)
+                                           cfg.l1_regularization, cfg.l2_regularization_categorical, w_inv=w_inv)
                     cnt = c[S.category_order(keys)]
                 else:
                     cnt = np.bincount(codes[rows].astype(np.int64), minlength=B)

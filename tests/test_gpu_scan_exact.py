@@ -42,13 +42,17 @@ def same_f32(a, b):
     return (np.isnan(a) and np.isnan(b)) or a == b
 
 
-def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1):
+def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1, sel=None, select=None):
     """Compares every captured candidate of the tree with the reference; -> number of (node, feature) pairs checked.
     `cols`: per feature (kind, codes or stored values, buckets, bucket values), kind 'num' / 'cat' (byte), 'wide_num' /
-    'wide_cat' (uint16), 'pre' (presorted).  `w`: example weights (the rows then carry w*g in `g`)."""
+    'wide_cat' (uint16), 'pre' (presorted).  `w`: example weights (the rows then carry w*g in `g`).  `sel`: the rows the
+    tree was trained on (subsample / GOSS; None: all).  `select(level, j, cap)`: the feature node j of the level must
+    split on (-1: none), in place of the first maximum in feature order (candidate sampling)."""
     wide = list(getattr(gbt.dataset, "wide", {}))
     sets = gbt.get_category_sets(tree_index, tree) if any(c[0] == "wide_cat" for c in cols) else {}
     rows_of = route(tree, cols, sets)
+    if sel is not None:
+        rows_of = {i: r[sel[r]] for i, r in rows_of.items()}
     min_obs = cfg.min_examples if cfg.in_split_min_examples_check else 1
     use_h = bool(cfg.use_hessian_gain)
     checked, derived_seen = 0, 0
@@ -111,8 +115,10 @@ def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1):
                         if kind == "cat":
                             ok = np.array_equal(want[:8], cap["cat_mask"][j, f])
                         else:
+                            # (the captured row is as wide as the widest wide categorical column)
                             got = cap["sets"][j, wide.index(f)]
-                            ok = np.array_equal(want[:len(got)], got) and not want[len(got):].any()
+                            m = max(len(want), len(got))
+                            ok = np.array_equal(np.pad(want, (0, m - len(want))), np.pad(got, (0, m - len(got))))
                         ok = ok and np.isnan(cap["threshold_value"][j, f])
                     else:
                         if kind == "pre":
@@ -131,9 +137,13 @@ def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1):
                     got = float(cap["score"][j, f])
                     assert abs(got - float(want)) <= ulp32(want), f"{where}: score {got} vs exact {float(v.exact)}"
             # the selection: the first maximum of the float scores in feature order, if > 0
-            sc = np.where(cap["found"][j] != 0, cap["score"][j], 0.0).astype(np.float32)
-            best = int(np.argmax(sc))
-            assert tree[pre]["feature"] == (best if sc[best] > 0 else -1), f"level {level} node {pre}: selection"
+            if select is not None:
+                want = select(level, j, cap)
+            else:
+                sc = np.where(cap["found"][j] != 0, cap["score"][j], 0.0).astype(np.float32)
+                best = int(np.argmax(sc))
+                want = best if sc[best] > 0 else -1
+            assert tree[pre]["feature"] == want, f"level {level} node {pre}: selection"
     if cfg.sibling_subtraction and cfg.max_depth > 2 and (tree["depth"] >= 3).any():
         assert derived_seen > 0
     return checked

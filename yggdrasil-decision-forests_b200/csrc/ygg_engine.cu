@@ -3127,7 +3127,8 @@ int ygg_gbt_set_validation_f32(ygg_gbt* h, const ygg_dataset* valid, const float
 int ygg_gbt_validation_loss(ygg_gbt* h, int32_t iter, float* loss, float* secondary) {
   if (!h || !loss || !secondary) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (h->vds == nullptr) return set_error(YGG_ERR_INVALID_ARGUMENT, "no validation rows attached");
-  if (iter < 0 || iter >= h->iters_done) return set_error(YGG_ERR_INVALID_ARGUMENT, "iteration %d not trained", iter);
+  // early stopping trains whole batches: the iterations past the stopping point are not logged
+  if (iter < 0 || iter >= ygg_gbt_num_iterations(h)) return set_error(YGG_ERR_INVALID_ARGUMENT, "iteration %d not logged", iter);
   YGG_CUDA(cudaSetDevice(h->ds->device));
   LossRec rec;
   YGG_CUDA(cudaMemcpyAsync(&rec, h->d_vloss + iter, sizeof(rec), cudaMemcpyDeviceToHost, h->stream));
@@ -3396,7 +3397,7 @@ int ygg_gbt_get_category_set(ygg_gbt* h, int32_t iter, int32_t node, uint32_t* w
 
 int ygg_gbt_train_loss(ygg_gbt* h, int32_t iter, float* loss, float* secondary) {
   if (!h || !loss || !secondary) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
-  if (iter < 0 || iter >= h->iters_done) return set_error(YGG_ERR_INVALID_ARGUMENT, "iteration %d not trained", iter);
+  if (iter < 0 || iter >= ygg_gbt_num_iterations(h)) return set_error(YGG_ERR_INVALID_ARGUMENT, "iteration %d not logged", iter);
   YGG_CUDA(cudaSetDevice(h->ds->device));
   YGG_RETURN_IF_ERROR(apply_pending(h));
   YGG_RETURN_IF_ERROR(reduce_losses(h));
