@@ -395,6 +395,31 @@ int ygg_num_candidate_attributes(int32_t num_features, int32_t loss, int32_t num
 uint64_t ygg_candidate_key(uint32_t random_seed, int32_t tree, int32_t node, int32_t feature);
 int ygg_gbt_set_candidate_sampling(ygg_gbt* h, int32_t num_candidate_attributes, float num_candidate_attributes_ratio);
 
+/* DART (GradientBoostedTreesTrainingConfig.dart, DESIGN.md §24): at the start of iteration i > 0 every earlier iteration
+ * is dropped with probability dropout_rate (one draw each from the learner's random stream; none dropped: one drawn
+ * uniformly), the iteration's gradients are taken at the predictions without the dropped trees, and after its trees the
+ * new iteration gets weight 1 / (|D| + 1) while the dropped ones are scaled by |D| / (|D| + 1).  Under DART the reference
+ * defaults shrinkage to 1.0 when it is not set; this ABI takes cfg.shrinkage as given.
+ *
+ * ygg_gbt_set_dart: after ygg_gbt_create, before the first tree.  INVALID_ARGUMENT for a NaN rate, one outside [0, 1], or
+ * after the first tree; YGG_ERR_UNIMPLEMENTED on a feature or row shard (either call order: the shard setters refuse a
+ * DART handle), and from ygg_gbt_set_predictions.  A ygg_gbt_step that fails after its DART draws leaves the handle unable
+ * to train further (the next step returns INVALID_ARGUMENT); its trees and model so far stay readable.  Allocates the leaf-id history of every tree: tree capacity x rows x 2
+ * bytes for the training rows (10M rows, 300 trees: 6 GB) and the same for the held-out rows; a failed allocation returns
+ * YGG_ERR_CUDA with the byte count.
+ *
+ * ygg_gbt_get_tree returns the trees as grown (unscaled leaves).  ygg_gbt_predict and ygg_gbt_save_ydf use the SCALED
+ * model: each leaf of iteration j becomes leaf * w_j (internal nodes unchanged), summed in tree order.
+ * ygg_gbt_get_predictions returns the training accumulator: the same model, but built by the per-iteration updates, so
+ * it is not bitwise equal to the scaled model's sum (the operations are in another order).
+ *
+ * ygg_gbt_get_dart_weights: the per-iteration weights w_j, one per iteration; after ygg_gbt_train they are the final
+ * model's (early stopping: the weights at the stop, for the iterations the model keeps).  ygg_gbt_get_dart_dropped: the
+ * dropped iterations of iteration `iter`, ascending. */
+int ygg_gbt_set_dart(ygg_gbt* h, float dropout_rate);
+int ygg_gbt_get_dart_weights(ygg_gbt* h, float* out, int32_t capacity, int32_t* n);
+int ygg_gbt_get_dart_dropped(ygg_gbt* h, int32_t iter, int32_t* out, int32_t capacity, int32_t* n);
+
 /* Copies tree `iter` (pre-order: node, neg subtree, pos subtree).  *n_nodes receives the node
  * count; fails with INVALID_ARGUMENT if capacity is too small. */
 int ygg_gbt_get_tree(ygg_gbt* h, int32_t iter, ygg_node* out, int32_t capacity, int32_t* n_nodes);

@@ -90,6 +90,7 @@ EXPORTS = [
     "ygg_dataset_set_numerical_column", "ygg_dataset_get_numerical_column",
     "ygg_debug_capture_candidates", "ygg_debug_level_candidates",
     "ygg_num_candidate_attributes", "ygg_candidate_key", "ygg_gbt_set_candidate_sampling", "ygg_debug_level_tried",
+    "ygg_gbt_set_dart", "ygg_gbt_get_dart_weights", "ygg_gbt_get_dart_dropped",
 ]
 
 
@@ -740,6 +741,26 @@ class Gbt:
         keyed order; ratio None: not set.  Before the first tree."""
         check(lib().ygg_gbt_set_candidate_sampling(self.handle, C.c_int32(int(num_candidate_attributes)),
                                                    C.c_float(-1.0 if ratio is None else float(ratio))))
+
+    def set_dart(self, dropout_rate):
+        """DART (ygg_gbt_set_dart): per-iteration dropout of earlier iterations at `dropout_rate`.  Before the first tree."""
+        check(lib().ygg_gbt_set_dart(self.handle, C.c_float(float(dropout_rate))))
+
+    def dart_weights(self):
+        """The per-iteration DART weights (float32 [iterations]); after train(), the final model's."""
+        n = C.c_int32()
+        cap = int(self.cfg.num_trees)
+        out = np.zeros(max(cap, 1), np.float32)
+        check(lib().ygg_gbt_get_dart_weights(self.handle, ptr(out, C.c_float), C.c_int32(cap), C.byref(n)))
+        return out[:n.value].copy()
+
+    def dart_dropped(self, it):
+        """The iterations dropped at iteration `it` (int32, ascending)."""
+        n = C.c_int32()
+        out = np.zeros(max(int(it), 1), np.int32)
+        check(lib().ygg_gbt_get_dart_dropped(self.handle, C.c_int32(int(it)), ptr(out, C.c_int32), C.c_int32(len(out)),
+                                             C.byref(n)))
+        return out[:n.value].copy()
 
     def level_tried(self, level):
         """The validity flags of tree level `level` of the last captured tree (sampling set before capture_candidates):

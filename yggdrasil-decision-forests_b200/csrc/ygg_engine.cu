@@ -217,6 +217,19 @@ struct ygg_gbt {
   // with the single-thread manager; 0: off), the scan's validity flags [split-level nodes][f_scan]
   int sample_k_valid = 0;
   uint8_t* d_tried = nullptr;
+  // DART (ygg_gbt_set_dart, DESIGN.md §24): d_pred / d_vpred hold the accumulators of the full predictions.  Per tree the
+  // leaf id of every training / held-out row ([tree capacity][n]) and its leaf values by node id ([tree capacity][max_nodes]);
+  // the dropped lists of the last two iterations (index i & 1, [iteration capacity] each); on the host every iteration's
+  // dropped set, new weight and sf - 1, and the weights after the last iteration trained.
+  bool dart = false;
+  float dart_rate = 0.f;
+  uint16_t* d_dart_hist = nullptr;
+  uint16_t* d_dart_vhist = nullptr;
+  float* d_dart_leaf = nullptr;
+  DartDrop* d_dart_list[2] = {nullptr, nullptr};
+  std::vector<std::vector<int32_t>> dart_dropped;
+  std::vector<float> dart_w_new, dart_sf_m1, dart_w;
+  std::vector<DartDrop> dart_host_list;
   // split-candidate capture (ygg_debug_capture_candidates): per level of the last tree, [num_levels] copies of the scan
   // phase's tables (d_cand, d_cand_mask, d_wide_thr, d_wide_set), of the node table, the level's families and descriptor
   struct Capture {
@@ -1542,8 +1555,9 @@ struct McParams {
   const float* weight;
   float* g2w;               // [K][n_pad]
   float correct_scale;
+  DartParams dart;          // DART instantiation: the gradients are taken at the sampled predictions (dart.smp)
 };
-template <bool WEIGHTED>
+template <bool WEIGHTED, bool DART = false>
 __global__ void __launch_bounds__(256) k_mc_grad(McParams p) {
   double loss = 0;
   unsigned long long correct = 0;
@@ -1566,6 +1580,14 @@ __global__ void __launch_bounds__(256) k_mc_grad(McParams p) {
       const float term = log_rn(e[label] / sum_exp);                  // :268-272
       loss -= WEIGHTED ? w * term : term;
       if (predicted == label) correct += WEIGHTED ? static_cast<unsigned long long>(__float2ull_rn(w * p.correct_scale)) : 1ull;
+    }
+    if (DART && p.g != nullptr && p.dart.n_smp > 0) {
+      sum_exp = 0.f;
+      for (int k = 0; k < p.K; k++) {
+        const float v = exp_rn(dart_sample(p.dart, p.pred[static_cast<int64_t>(k) * p.n + r], k, r));
+        e[k] = v;
+        sum_exp += v;
+      }
     }
     if (p.g != nullptr) {
       const float normalization = 1.f / sum_exp;                      // TemplatedUpdateGradients :163-189
@@ -1605,6 +1627,23 @@ __global__ void __launch_bounds__(256) k_apply_leaves(float* __restrict__ pred, 
     pred[r] += tree[node_of_row[r]].leaf_value;
 }
 
+// DART, multinomial: the update of the tree just grown on its class plane (d.plane), its rows' leaf ids into the history.
+__global__ void __launch_bounds__(256) k_dart_apply(float* __restrict__ pred, const uint16_t* __restrict__ node_of_row,
+                                                    const NodeRec* __restrict__ tree, int64_t n, DartParams d) {
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n; r += stride) {
+    const uint16_t node = node_of_row[r];
+    d.hist[static_cast<int64_t>(d.upd_tree) * d.n + r] = node;
+    pred[r] = dart_update(d, pred[r], tree[node].leaf_value, d.plane, r);
+  }
+}
+
+// DART: the leaf values of a finished tree by node id, the compact table the dropped-tree gathers read.
+__global__ void k_dart_leaves(const NodeRec* __restrict__ tree, int max_nodes, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < max_nodes) out[i] = tree[i].leaf_value;
+}
+
 // Validation rows: UpdatePredictions on the held-out rows by tree traversal (loss_utils.cc:214-229,
 // gradient_boosted_trees.cc:1556-1566) fused with the validation loss of the iteration
 // (:1610-1626; loss_imp_binomial.cc:204-234, metric/metric.cc:2173-2199).
@@ -1621,7 +1660,9 @@ __device__ __forceinline__ uint32_t row_bin(const uint8_t* __restrict__ bins, co
   return wi >= 0 ? wide[static_cast<int64_t>(wi) * n_pad + r] : bins[static_cast<int64_t>(f) * n_pad + r];
 }
 
-template <int LOSS>
+// DART: the held-out rows' own accumulator takes the DART update of the iteration, and each row's leaf id goes into the
+// validation history (`dart`).
+template <int LOSS, bool DART = false>
 __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
                                                       const int32_t* __restrict__ wide_of, const float* __restrict__ num,
                                                       const int32_t* __restrict__ num_of, int64_t n, int64_t n_pad,
@@ -1629,7 +1670,7 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
                                                       int set_words, float* __restrict__ pred,
                                                       const uint8_t* __restrict__ label_u8,
                                                       const float* __restrict__ label_f32, LossRec* out, LossPartials* partials,
-                                                      const float* __restrict__ weight, float correct_scale) {
+                                                      const float* __restrict__ weight, float correct_scale, DartParams dart) {
   double loss = 0;
   unsigned long long correct = 0;
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
@@ -1643,7 +1684,13 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
       const bool pos = split_goes_pos(tree[node], b, wide_split, sets + static_cast<size_t>(node) * set_words);
       node = pos ? tree[node].pos_child : tree[node].neg_child;
     }
-    const float p = pred[r] + tree[node].leaf_value;
+    float p;
+    if (DART) {
+      dart.hist[static_cast<int64_t>(dart.upd_tree) * dart.n + r] = static_cast<uint16_t>(node);
+      p = dart_update(dart, pred[r], tree[node].leaf_value, dart.plane, r);
+    } else {
+      p = pred[r] + tree[node].leaf_value;
+    }
     pred[r] = p;
     if (LOSS == 2) continue;  // multinomial: the loss needs all K planes (k_mc_grad after the K-th tree)
     if (LOSS == 0) {
@@ -1679,11 +1726,13 @@ __global__ void __launch_bounds__(256) k_valid_update(const uint8_t* __restrict_
 // Raw scores of the model's first `n_trees` trees on any dataset with the training dataset's features (ComputePredictions,
 // gradient_boosted_trees.cc:2872-2930: the predictions a resumed training starts from): initial prediction + the leaves
 // reached in every tree of the row's class plane.  One thread per row, trees in order (float sums in the reference's order).
+// SCALED (DART): the leaf of a tree of iteration j counts as the rounded product leaf * scale[j], the model's scaled leaf.
+template <bool SCALED = false>
 __global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bins, const uint16_t* __restrict__ wide,
                                                 const int32_t* __restrict__ wide_of, const float* __restrict__ num,
                                                 const int32_t* __restrict__ num_of, int64_t n, int64_t n_pad, const NodeRec* __restrict__ trees,
                                                 const uint32_t* __restrict__ sets, int set_words, int pool_nodes, int max_nodes, int n_trees, int K,
-                                                float initial, float* __restrict__ out /*[K][n]*/) {
+                                                float initial, float* __restrict__ out /*[K][n]*/, const float* __restrict__ scale) {
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n; r += stride) {
     for (int k = 0; k < K; k++) {
@@ -1700,11 +1749,38 @@ __global__ void __launch_bounds__(256) k_predict(const uint8_t* __restrict__ bin
                                           sets + (static_cast<size_t>(t) * pool_nodes + node) * set_words);
           node = pos ? tree[node].pos_child : tree[node].neg_child;
         }
-        acc += tree[node].leaf_value;
+        if (SCALED) acc = __fadd_rn(acc, __fmul_rn(tree[node].leaf_value, scale[t / K]));
+        else acc += tree[node].leaf_value;
       }
       out[static_cast<int64_t>(k) * n + r] = acc;
     }
   }
+}
+
+// The DART state of a launch: `upd_iter` the iteration whose update is applied (tree upd_iter * K + plane; -1: none),
+// `smp_iter` the iteration whose sampled predictions are formed (-1: none), on the training or the held-out rows.  The
+// device lists of both iterations must still be in their slots (index & 1).
+DartParams dart_params(const ygg_gbt* h, int upd_iter, int plane, int smp_iter, bool valid) {
+  DartParams d{};
+  d.hist = valid ? h->d_dart_vhist : h->d_dart_hist;
+  d.leaf = h->d_dart_leaf;
+  d.n = valid ? h->vds->n : h->ds->n;
+  d.max_nodes = h->max_nodes;
+  d.K = h->K;
+  d.plane = plane;
+  d.upd_tree = -1;
+  if (upd_iter >= 0) {
+    d.upd_tree = upd_iter * h->K + plane;
+    d.upd = h->d_dart_list[upd_iter & 1];
+    d.n_upd = static_cast<int>(h->dart_dropped[upd_iter].size());
+    d.w_new = h->dart_w_new[upd_iter];
+    d.sf_m1 = h->dart_sf_m1[upd_iter];
+  }
+  if (smp_iter >= 0) {
+    d.smp = h->d_dart_list[smp_iter & 1];
+    d.n_smp = static_cast<int>(h->dart_dropped[smp_iter].size());
+  }
+  return d;
 }
 
 // `tree_idx`: the tree just grown; `plane`: its class (0 unless multinomial).
@@ -1714,9 +1790,14 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
   const NodeRec* tree = h->d_nodes_all + static_cast<size_t>(tree_idx) * h->max_nodes;
   const int64_t nv = h->vds->n;
   const int grid = static_cast<int>(std::min<int64_t>((nv + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 8));
+  const DartParams dart = h->dart ? dart_params(h, h->iters_done, plane, -1, true) : DartParams{};
   if (is_multinomial(h)) {
-    k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred + static_cast<int64_t>(plane) * nv,
-                                                   nullptr, nullptr, nullptr, nullptr, nullptr, 0.f);
+    if (h->dart)
+      k_valid_update<2, true><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred + static_cast<int64_t>(plane) * nv,
+                                                           nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, dart);
+    else
+      k_valid_update<2><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred + static_cast<int64_t>(plane) * nv,
+                                                     nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, dart);
     h->launches_total++;
     YGG_RETURN_IF_ERROR(check_launch("k_valid_update"));
     if (plane + 1 == h->K) {  // all K trees of the iteration applied: validation loss of the iteration
@@ -1731,14 +1812,11 @@ int launch_valid_update(ygg_gbt* h, int tree_idx, int plane = 0) {
     }
     return YGG_OK;
   }
-  if (h->cfg.loss == YGG_LOSS_BINOMIAL_LOG_LIKELIHOOD)
-    k_valid_update<0><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
-                                                   h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
-                                                   h->d_vweight, h->v_correct_scale);
-  else
-    k_valid_update<1><<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
-                                                   h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
-                                                   h->d_vweight, h->v_correct_scale);
+  const bool binomial = h->cfg.loss == YGG_LOSS_BINOMIAL_LOG_LIKELIHOOD;
+  auto kernel = binomial ? (h->dart ? k_valid_update<0, true> : k_valid_update<0>) : (h->dart ? k_valid_update<1, true> : k_valid_update<1>);
+  kernel<<<grid, 256, 0, h->stream>>>(h->vds->d_bins, h->vds->d_wide, h->vds->d_wide_of, h->vds->d_num, h->vds->d_num_of, nv, h->vds->n_pad, tree, sets_of(h, tree), h->set_words, h->d_vpred, h->d_vlabel_u8,
+                                      h->d_vlabel_f32, h->d_vloss + h->iters_done, h->d_loss_partials,
+                                      h->d_vweight, h->v_correct_scale, dart);
   h->launches_total++;
   return check_launch("k_valid_update");
 }
@@ -1783,7 +1861,11 @@ int launch_mc(ygg_gbt* h, bool with_loss, bool with_grad) {
   p.out = with_loss ? h->d_loss + (h->iters_done - 1) : nullptr;
   p.partials = h->d_loss_partials;
   p.weight = h->d_weight; p.g2w = h->d_g2w; p.correct_scale = correct_scale_of(h->w_pow2);
-  if (user_weighted(h)) k_mc_grad<true><<<elementwise_grid(h), 256, 0, h->stream>>>(p);
+  if (h->dart && with_grad) {   // the loss at the full predictions, the gradients at this iteration's sampled ones
+    p.dart = dart_params(h, -1, 0, h->iters_done, false);
+    if (user_weighted(h)) k_mc_grad<true, true><<<elementwise_grid(h), 256, 0, h->stream>>>(p);
+    else k_mc_grad<false, true><<<elementwise_grid(h), 256, 0, h->stream>>>(p);
+  } else if (user_weighted(h)) k_mc_grad<true><<<elementwise_grid(h), 256, 0, h->stream>>>(p);
   else k_mc_grad<false><<<elementwise_grid(h), 256, 0, h->stream>>>(p);
   h->launches_total++;
   return check_launch("k_mc_grad");
@@ -1800,7 +1882,13 @@ int launch_pred_grad(ygg_gbt* h, bool apply, bool compute_grad) {
   g.weight = h->d_weight; g.g2w = h->d_g2w; g.correct_scale = correct_scale_of(h->w_pow2);
   if (apply) { k_reset_loss<<<1, 1, 0, h->stream>>>(h->d_st); h->launches_total++; }
   const bool binomial = h->cfg.loss == YGG_LOSS_BINOMIAL_LOG_LIKELIHOOD;
-  if (user_weighted(h)) {
+  if (h->dart) {
+    // the pending tree is the last one of iteration iters_done - 1; the gradients are those of iteration iters_done
+    g.dart = dart_params(h, apply ? h->iters_done - 1 : -1, 0, compute_grad ? h->iters_done : -1, false);
+    auto kernel = user_weighted(h) ? (binomial ? k_pred_grad<0, true, true> : k_pred_grad<1, true, true>)
+                                   : (binomial ? k_pred_grad<0, false, true> : k_pred_grad<1, false, true>);
+    kernel<<<elementwise_grid(h), 256, 0, h->stream>>>(g);
+  } else if (user_weighted(h)) {
     if (binomial) k_pred_grad<0, true><<<elementwise_grid(h), 256, 0, h->stream>>>(g);
     else k_pred_grad<1, true><<<elementwise_grid(h), 256, 0, h->stream>>>(g);
   } else if (binomial) k_pred_grad<0><<<elementwise_grid(h), 256, 0, h->stream>>>(g);
@@ -1859,6 +1947,17 @@ int check_device_error(ygg_gbt* h) {
   return YGG_OK;
 }
 
+// libc++'s uniform_int_distribution draw of [0, rp - 1], 1 <= rp <= 2^32: nothing drawn for rp == 1, else the low w bits
+// of one engine word, redrawn while >= rp.
+uint32_t uniform_int_libcxx(uint64_t rp, std::mt19937* g) {
+  if (rp == 1) return 0;
+  int w = 63 - __builtin_clzll(rp);
+  if (rp & ((1ull << w) - 1)) ++w;
+  uint32_t u;
+  do { u = (*g)() & static_cast<uint32_t>((1ull << w) - 1); } while (u >= rp);
+  return u;
+}
+
 // libc++'s std::shuffle (llvm libcxx/include/__algorithm/shuffle.h): for every position but the last, draw i in [0, d]
 // with its uniform_int_distribution — the low w bits of one engine word, redrawn while > d (w = bits of d + 1) — and
 // swap.  The reference's golden models were built against libc++ (DESIGN.md §6); libstdc++'s differs.
@@ -1866,11 +1965,7 @@ void shuffle_libcxx(std::vector<int32_t>* v, std::mt19937* g) {
   const int64_t n = static_cast<int64_t>(v->size());
   int64_t d = n - 1;
   for (int64_t first = 0; first < n - 1; ++first, --d) {
-    const uint64_t rp = static_cast<uint64_t>(d) + 1;
-    int w = 63 - __builtin_clzll(rp);
-    if (rp & ((1ull << w) - 1)) ++w;
-    uint32_t u;
-    do { u = (*g)() & static_cast<uint32_t>((1ull << w) - 1); } while (u >= rp);
+    const uint32_t u = uniform_int_libcxx(static_cast<uint64_t>(d) + 1, g);
     if (u != 0) std::swap((*v)[first], (*v)[first + u]);
   }
 }
@@ -2014,6 +2109,75 @@ int draw_goss(ygg_gbt* h) {
   h->goss_cutoff = cutoff;
   h->n_selected = count;
   return YGG_OK;
+}
+
+// DART, host part (DartPredictionAccumulator::SampleIterIndices, gradient_boosted_trees.cc:3108-3130): at the start of
+// iteration i > 0, before the gradient and row-sampling draws, one std::uniform_real_distribution<float> word per earlier
+// iteration, dropped iff < dropout_rate; an empty set takes one iteration drawn uniformly (libc++'s or libstdc++'s
+// uniform_int_distribution, as the tie-break replay's shuffle).  Uploads the dropped list with the weights before this
+// iteration's update, then applies the update to the host weights: w_j *= sf for the dropped, 1 / (|D| + 1) for the new.
+int draw_dart(ygg_gbt* h) {
+  if (h->cfg.candidate_shuffle != 0) YGG_RETURN_IF_ERROR(resolve_ties(h, h->trees_done));
+  ensure_tie_rng(h);
+  const int i = h->iters_done;
+  std::vector<int32_t> dropped;
+  if (i > 0) {
+    std::uniform_real_distribution<float> unif_dist_unit;
+    for (int j = 0; j < i; j++)
+      if (unif_dist_unit(h->tie_rng) < h->dart_rate) dropped.push_back(j);
+    if (dropped.empty())
+      dropped.push_back(h->cfg.candidate_shuffle == 2 ? static_cast<int32_t>(uniform_int_libcxx(static_cast<uint64_t>(i), &h->tie_rng))
+                                                      : std::uniform_int_distribution<int>(0, i - 1)(h->tie_rng));
+  }
+  h->dart_host_list.clear();
+  for (int32_t j : dropped) h->dart_host_list.push_back({j, h->dart_w[j]});
+  if (!dropped.empty())
+    YGG_CUDA(cudaMemcpyAsync(h->d_dart_list[i & 1], h->dart_host_list.data(), sizeof(DartDrop) * dropped.size(),
+                             cudaMemcpyHostToDevice, h->stream));
+  // (gradient_boosted_trees.cc:3165-3214) every operation rounded to float
+  const float denom = static_cast<float>(dropped.size() + 1);
+  const float w_new = 1.f / denom;
+  const float sf = static_cast<float>(dropped.size()) / denom;
+  for (int32_t j : dropped) h->dart_w[j] = h->dart_w[j] * sf;
+  h->dart_w.push_back(w_new);
+  h->dart_w_new.push_back(w_new);
+  h->dart_sf_m1.push_back(sf - 1.f);
+  h->dart_dropped.push_back(std::move(dropped));
+  return YGG_OK;
+}
+
+// DART: the leaf values of the finished tree `trees_done` (`nodes`) into its row of the compact leaf table.
+int stage_dart_leaves(ygg_gbt* h, const NodeRec* nodes) {
+  ProfScope ps(h, "grad");
+  k_dart_leaves<<<(h->max_nodes + 255) / 256, 256, 0, h->stream>>>(nodes, h->max_nodes,
+                                                                    h->d_dart_leaf + static_cast<size_t>(h->trees_done) * h->max_nodes);
+  h->launches_total++;
+  return check_launch("k_dart_leaves");
+}
+
+// The DART weights of the first `iters` iterations as they are after iteration `iters` - 1: the updates replayed from the
+// dropped sets (the same float operations as draw_dart).
+std::vector<float> dart_weights_after(const ygg_gbt* h, int iters) {
+  std::vector<float> w;
+  for (int i = 0; i < iters; i++) {
+    const std::vector<int32_t>& dropped = h->dart_dropped[i];
+    const float denom = static_cast<float>(dropped.size() + 1);
+    const float sf = static_cast<float>(dropped.size()) / denom;
+    for (int32_t j : dropped) w[j] = w[j] * sf;
+    w.push_back(1.f / denom);
+  }
+  return w;
+}
+
+// The per-iteration leaf scales of the model: the weights as training stopped (the last iteration trained, also under
+// early stopping), for the iterations the model keeps.  Empty without DART.
+std::vector<float> dart_model_scales(const ygg_gbt* h) {
+  if (!h->dart) return {};
+  const int trees = h->final_trees >= 0 ? h->final_trees : h->trees_done;
+  const int trained = h->log_entries >= 0 ? h->log_entries : h->iters_done;
+  std::vector<float> w = dart_weights_after(h, trained);
+  w.resize(trees / h->K);
+  return w;
 }
 
 // Device part, after the iteration's unit gradients are in d_g / d_h: order the rows by decreasing |g| (stable: equal keys
@@ -2676,6 +2840,7 @@ int ygg_gbt_destroy(ygg_gbt* h) {
   dev_free(h->d_master_val); dev_free(h->d_master_row); dev_free(h->d_ps); dev_free(h->d_ph); dev_free(h->d_presort_temp);
   for (int i = 0; i < 2; i++) { dev_free(h->d_list_val[i]); dev_free(h->d_list_row[i]); }
   dev_free(h->d_seg_off); dev_free(h->d_seg_total); dev_free(h->d_sbest); dev_free(h->d_sbest_idx); dev_free(h->d_num_feature);
+  dev_free(h->d_dart_hist); dev_free(h->d_dart_vhist); dev_free(h->d_dart_leaf); dev_free(h->d_dart_list[0]); dev_free(h->d_dart_list[1]);
   free_capture(h);
   cudaFree(h->d_goss_temp);
   cudaFree(h->d_level_buf);
@@ -2703,6 +2868,7 @@ static int set_initial_predictions(ygg_gbt* h) {
   h->pending_loss = false;
   h->loss_reduced_upto = 0;
   h->pending = false;
+  h->dart_dropped.clear(); h->dart_w_new.clear(); h->dart_sf_m1.clear(); h->dart_w.clear();
   h->has_labels = true;
   return YGG_OK;
 }
@@ -2884,6 +3050,7 @@ int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature
   if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "shard must be set before training");
   if (world > 1 && h->cfg.candidate_shuffle != 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate_shuffle is not combined with sharding");
   if (h->sample_k_valid > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate feature sampling is not combined with sharding");
+  if (h->dart) return set_error(YGG_ERR_UNIMPLEMENTED, "DART is not combined with sharding");
   YGG_CUDA(cudaSetDevice(h->ds->device));
   h->f_begin = feature_begin; h->f_end = feature_end; h->rank = rank; h->world = world;
   h->hist_f_begin = feature_begin; h->hist_f_end = feature_end;
@@ -2909,6 +3076,7 @@ int ygg_gbt_set_row_shard(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_row
 
   if (world > 1 && h->cfg.candidate_shuffle != 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate_shuffle is not combined with sharding");
   if (h->sample_k_valid > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate feature sampling is not combined with sharding");
+  if (h->dart) return set_error(YGG_ERR_UNIMPLEMENTED, "DART is not combined with sharding");
   if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "shard must be set before training");
   YGG_CUDA(cudaSetDevice(h->ds->device));
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
@@ -2990,6 +3158,18 @@ __global__ void k_gather_rows16(const uint16_t* __restrict__ in, int64_t in_pad,
     out[static_cast<int64_t>(f) * out_pad + i] = in[static_cast<int64_t>(f) * in_pad + rows[i]];
 }
 
+// DART: the leaf-id history of `rows` rows, u16 [tree capacity][rows].
+int alloc_dart_history(ygg_gbt* h, uint16_t** p, int64_t rows, const char* what) {
+  const size_t elems = static_cast<size_t>(h->tree_capacity) * static_cast<size_t>(rows);
+  if (dev_alloc(p, elems) != YGG_OK) {
+    (void)cudaGetLastError();
+    *p = nullptr;
+    return set_error(YGG_ERR_CUDA, "DART: %zu bytes of leaf history (%d trees x %lld %s rows x 2 B) could not be allocated",
+                     elems * sizeof(uint16_t), h->tree_capacity, static_cast<long long>(rows), what);
+  }
+  return YGG_OK;
+}
+
 int attach_validation(ygg_gbt* h, const ygg_dataset* valid, int64_t n) {
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
   if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "validation rows must be attached before training");
@@ -3006,6 +3186,11 @@ int attach_validation(ygg_gbt* h, const ygg_dataset* valid, int64_t n) {
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_vpred, n * h->K));
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_vloss, h->tree_capacity));
   YGG_CUDA(cudaMemsetAsync(h->d_vloss, 0, sizeof(LossRec) * h->tree_capacity, h->stream));
+  if (h->dart) {
+    dev_free(h->d_dart_vhist);
+    h->d_dart_vhist = nullptr;
+    YGG_RETURN_IF_ERROR(alloc_dart_history(h, &h->d_dart_vhist, n, "held-out"));
+  }
   // the validation predictions start from the initial prediction of the TRAINING rows
   k_fill<<<static_cast<int>(std::min<int64_t>((n + 255) / 256, 4096)), 256, 0, h->stream>>>(h->d_vpred, n * h->K, h->initial_prediction);
   h->launches_total++;
@@ -3182,6 +3367,11 @@ int ygg_gbt_step(ygg_gbt* h) {
   if (h->finalized) return set_error(YGG_ERR_INVALID_ARGUMENT, "training was finalized by early stopping");
   YGG_CUDA(cudaSetDevice(h->ds->device));
   (void)cudaGetLastError();  // drop a stale, non-sticky error of an earlier foreign runtime call (see check_launch)
+  // a DART iteration that failed after its draws has advanced the dropped sets, the weights and the random stream: the
+  // handle cannot train on consistently
+  if (h->dart && h->dart_dropped.size() != static_cast<size_t>(h->iters_done))
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "an earlier DART iteration failed part-way: the handle cannot continue training");
+  if (h->dart) YGG_RETURN_IF_ERROR(draw_dart(h));
   if (goss(h)) YGG_RETURN_IF_ERROR(draw_goss(h));
   else if (sampling(h)) YGG_RETURN_IF_ERROR(draw_sample(h));
   const int64_t n_job = sampling(h) ? h->n_selected : (h->shard_mode == kShardRows ? h->n_global : h->ds->n);
@@ -3208,10 +3398,19 @@ int ygg_gbt_step(ygg_gbt* h) {
       NodeRec* nodes = h->d_nodes_all + static_cast<size_t>(h->trees_done) * h->max_nodes;
       YGG_RETURN_IF_ERROR(grow_tree(h, nodes));
       if (h->cfg.growing_strategy == 1) YGG_RETURN_IF_ERROR(best_first_prune(h, nodes));
-      k_apply_leaves<<<elementwise_grid(h), 256, 0, h->stream>>>(h->d_pred + static_cast<int64_t>(k) * h->ds->n, h->d_node_of_row,
-                                                                 nodes, h->ds->n);
-      h->launches_total++;
-      YGG_RETURN_IF_ERROR(check_launch("k_apply_leaves"));
+      if (h->dart) {
+        YGG_RETURN_IF_ERROR(stage_dart_leaves(h, nodes));
+        ProfScope ps(h, "grad");
+        k_dart_apply<<<elementwise_grid(h), 256, 0, h->stream>>>(h->d_pred + static_cast<int64_t>(k) * h->ds->n, h->d_node_of_row,
+                                                                 nodes, h->ds->n, dart_params(h, h->iters_done, k, -1, false));
+        h->launches_total++;
+        YGG_RETURN_IF_ERROR(check_launch("k_dart_apply"));
+      } else {
+        k_apply_leaves<<<elementwise_grid(h), 256, 0, h->stream>>>(h->d_pred + static_cast<int64_t>(k) * h->ds->n, h->d_node_of_row,
+                                                                   nodes, h->ds->n);
+        h->launches_total++;
+        YGG_RETURN_IF_ERROR(check_launch("k_apply_leaves"));
+      }
       if (h->vds != nullptr && h->cfg.candidate_shuffle != 0) { h->trees_done++; const int st = resolve_ties(h, h->trees_done); h->trees_done--; YGG_RETURN_IF_ERROR(st); }
       YGG_RETURN_IF_ERROR(launch_valid_update(h, h->trees_done, k));
       h->trees_done++;
@@ -3237,6 +3436,7 @@ int ygg_gbt_step(ygg_gbt* h) {
   NodeRec* nodes = h->d_nodes_all + static_cast<size_t>(h->trees_done) * h->max_nodes;
   YGG_RETURN_IF_ERROR(grow_tree(h, nodes));
   if (h->cfg.growing_strategy == 1) YGG_RETURN_IF_ERROR(best_first_prune(h, nodes));
+  if (h->dart) YGG_RETURN_IF_ERROR(stage_dart_leaves(h, nodes));
   // held-out rows are routed by the FINAL conditions: twins agree on the training rows only
   if (h->vds != nullptr && h->cfg.candidate_shuffle != 0) { h->trees_done++; const int st = resolve_ties(h, h->trees_done); h->trees_done--; YGG_RETURN_IF_ERROR(st); }
   YGG_RETURN_IF_ERROR(launch_valid_update(h, h->trees_done));
@@ -3433,19 +3633,32 @@ int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   float* d_out = nullptr;
   YGG_RETURN_IF_ERROR(dev_alloc(&d_out, static_cast<size_t>(n)));
   const int n_trees = ygg_gbt_num_trees(h);
-  k_predict<<<static_cast<int>(std::min<int64_t>((ds->n + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 16)), 256, 0, h->stream>>>(
-      ds->d_bins, ds->d_wide, ds->d_wide_of, ds->d_num, ds->d_num_of, ds->n, ds->n_pad, h->d_nodes_all, h->d_sets, h->set_words, pool_nodes(h), h->max_nodes, n_trees, h->K, h->initial_prediction, d_out);
+  float* d_scale = nullptr;
+  if (h->dart) {   // the scaled model: every leaf of iteration j times w_j
+    const std::vector<float> scale = dart_model_scales(h);
+    int st = dev_alloc(&d_scale, scale.size());
+    if (st == YGG_OK && !scale.empty() &&
+        cudaMemcpyAsync(d_scale, scale.data(), sizeof(float) * scale.size(), cudaMemcpyHostToDevice, h->stream) != cudaSuccess)
+      st = set_error(YGG_ERR_CUDA, "upload of the DART weights failed: %s", cudaGetErrorString(cudaGetLastError()));
+    if (st != YGG_OK) { dev_free(d_out); dev_free(d_scale); return st; }
+  }
+  const int grid = static_cast<int>(std::min<int64_t>((ds->n + 255) / 256, static_cast<int64_t>(h->ds->num_sms) * 16));
+  auto kernel = h->dart ? k_predict<true> : k_predict<false>;
+  kernel<<<grid, 256, 0, h->stream>>>(ds->d_bins, ds->d_wide, ds->d_wide_of, ds->d_num, ds->d_num_of, ds->n, ds->n_pad, h->d_nodes_all, h->d_sets,
+                                      h->set_words, pool_nodes(h), h->max_nodes, n_trees, h->K, h->initial_prediction, d_out, d_scale);
   h->launches_total++;
   int st = check_launch("k_predict");
   if (st == YGG_OK && (cudaMemcpyAsync(out, d_out, sizeof(float) * n, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
                        cudaStreamSynchronize(h->stream) != cudaSuccess))
     st = set_error(YGG_ERR_CUDA, "prediction read-back failed: %s", cudaGetErrorString(cudaGetLastError()));
   dev_free(d_out);
+  dev_free(d_scale);
   return st;
 }
 
 int ygg_gbt_set_predictions(ygg_gbt* h, const float* pred, int64_t n) {
   if (!h || !pred) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (h->dart) return set_error(YGG_ERR_UNIMPLEMENTED, "DART keeps its own accumulator of the predictions: not combined with ygg_gbt_set_predictions");
   if (n != h->ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "n mismatch");
   YGG_CUDA(cudaSetDevice(h->ds->device));
   YGG_RETURN_IF_ERROR(apply_pending(h));
@@ -3939,6 +4152,49 @@ int ygg_gbt_set_candidate_sampling(ygg_gbt* h, int32_t num_candidate_attributes,
   return YGG_OK;
 }
 
+int ygg_gbt_set_dart(ygg_gbt* h, float dropout_rate) {
+  if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
+  if (std::isnan(dropout_rate) || dropout_rate < 0.f || dropout_rate > 1.f)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "dart dropout_rate=%g outside [0, 1]", dropout_rate);
+  if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "DART must be set before training");
+  if (h->shard_mode != kShardNone || h->f_begin != 0 || h->f_end != h->ds->F)
+    return set_error(YGG_ERR_UNIMPLEMENTED, "DART is not combined with sharding");
+  YGG_CUDA(cudaSetDevice(h->ds->device));
+  (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
+  // (a call that failed part-way keeps what it allocated: a retry completes it)
+  if (h->d_dart_hist == nullptr) YGG_RETURN_IF_ERROR(alloc_dart_history(h, &h->d_dart_hist, h->ds->n, "training"));
+  if (h->vds != nullptr && h->d_dart_vhist == nullptr)
+    YGG_RETURN_IF_ERROR(alloc_dart_history(h, &h->d_dart_vhist, h->vds->n, "held-out"));
+  if (h->d_dart_leaf == nullptr) YGG_RETURN_IF_ERROR(dev_alloc(&h->d_dart_leaf, static_cast<size_t>(h->tree_capacity) * h->max_nodes));
+  for (int i = 0; i < 2; i++)
+    if (h->d_dart_list[i] == nullptr) YGG_RETURN_IF_ERROR(dev_alloc(&h->d_dart_list[i], static_cast<size_t>(h->cfg.num_trees)));
+  h->dart = true;
+  h->dart_rate = dropout_rate;
+  return YGG_OK;
+}
+
+int ygg_gbt_get_dart_weights(ygg_gbt* h, float* out, int32_t capacity, int32_t* n) {
+  if (!h || !n) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (!h->dart) return set_error(YGG_ERR_INVALID_ARGUMENT, "DART is not enabled on this handle");
+  const std::vector<float> w = h->finalized ? dart_model_scales(h) : h->dart_w;
+  *n = static_cast<int32_t>(w.size());
+  if (*n > capacity || (!out && *n > 0)) return set_error(YGG_ERR_INVALID_ARGUMENT, "capacity %d < %d weights", capacity, *n);
+  if (*n > 0) std::memcpy(out, w.data(), sizeof(float) * w.size());
+  return YGG_OK;
+}
+
+int ygg_gbt_get_dart_dropped(ygg_gbt* h, int32_t iter, int32_t* out, int32_t capacity, int32_t* n) {
+  if (!h || !n) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  if (!h->dart) return set_error(YGG_ERR_INVALID_ARGUMENT, "DART is not enabled on this handle");
+  if (iter < 0 || iter >= static_cast<int32_t>(h->dart_dropped.size()))
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "iteration %d not trained (have %zu)", iter, h->dart_dropped.size());
+  const std::vector<int32_t>& d = h->dart_dropped[iter];
+  *n = static_cast<int32_t>(d.size());
+  if (*n > capacity || (!out && *n > 0)) return set_error(YGG_ERR_INVALID_ARGUMENT, "capacity %d < %d dropped iterations", capacity, *n);
+  if (*n > 0) std::memcpy(out, d.data(), sizeof(int32_t) * d.size());
+  return YGG_OK;
+}
+
 int ygg_debug_level_tried(ygg_gbt* h, int32_t level, int32_t capacity, uint8_t* tried, int32_t* first_node, int32_t* n_nodes) {
   if (!h || !tried || !first_node || !n_nodes) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   const ygg_gbt::Capture& c = h->cap;
@@ -4011,10 +4267,14 @@ int ygg_gbt_save_ydf(ygg_gbt* h, const char* directory, const char* label_name, 
   for (int w = 0; w < ds->n_wide(); w++) num_values[ds->wide_feature[w]] = ds->wide_bins[w];
   std::vector<int64_t> set_offset;                  // wide categorical splits: their pooled sets
   std::vector<uint32_t> set_words;
+  const std::vector<float> dart_scale = dart_model_scales(h);
   for (int t = 0; t < n_trees; t++) {
     const NodeRec* d_tree = h->d_nodes_all + static_cast<size_t>(t) * h->max_nodes;
     std::vector<ygg_node> flat;
     YGG_RETURN_IF_ERROR(fetch_tree(h, d_tree, &flat));
+    if (h->dart)   // ScaleRegressorOutput (decision_tree.cc:1980-1988): the leaves only
+      for (ygg_node& nd : flat)
+        if (nd.feature < 0) nd.leaf_value = nd.leaf_value * dart_scale[t / h->K];
     if (h->d_sets != nullptr) {
       std::vector<NodeRec> nodes(h->max_nodes);
       std::vector<int> ids;

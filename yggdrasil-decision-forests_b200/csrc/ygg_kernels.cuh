@@ -85,6 +85,45 @@ __device__ __forceinline__ void reduce_loss_in_order(LossPartials* part, double 
   }
 }
 
+// DART (DESIGN.md §24).  One dropped iteration of a list: its index and its weight before the current update.
+struct DartDrop {
+  int32_t iter;
+  float w;
+};
+// The DART state a kernel reads: every tree's leaf id per row (`hist`, [trees][n]) and leaf values by node id (`leaf`,
+// [trees][max_nodes]); `upd`: the update of the iteration being applied (its dropped list, new weight, sf - 1), `smp`:
+// the dropped list of the iteration whose gradients are formed.  `K` trees per iteration, `plane`: the class of the tree
+// being applied (multinomial).
+struct DartParams {
+  uint16_t* hist;
+  const float* leaf;
+  int64_t n;
+  int max_nodes, K, plane;
+  int upd_tree;                 // tree whose leaf ids are stored (-1: none)
+  const DartDrop* upd;
+  int n_upd;
+  float w_new, sf_m1;
+  const DartDrop* smp;
+  int n_smp;
+};
+// p_j * w_j of dropped entry `e` for row r of class plane k.
+__device__ __forceinline__ float dart_term(const DartParams& d, const DartDrop& e, int k, int64_t r) {
+  const int64_t t = static_cast<int64_t>(e.iter) * d.K + k;
+  const float v = d.leaf[t * d.max_nodes + d.hist[t * d.n + r]];
+  return __fmul_rn(v, e.w);
+}
+// acc + p_i * w_new, then + (p_j * w_j) * (sf - 1) for every dropped j in ascending order: one rounding per operation.
+__device__ __forceinline__ float dart_update(const DartParams& d, float acc, float leaf, int k, int64_t r) {
+  acc = __fadd_rn(acc, __fmul_rn(leaf, d.w_new));
+  for (int i = 0; i < d.n_upd; i++) acc = __fadd_rn(acc, __fmul_rn(dart_term(d, d.upd[i], k, r), d.sf_m1));
+  return acc;
+}
+// The sampled prediction: acc - p_j * w_j for every dropped j in ascending order.
+__device__ __forceinline__ float dart_sample(const DartParams& d, float acc, int k, int64_t r) {
+  for (int i = 0; i < d.n_smp; i++) acc = __fsub_rn(acc, dart_term(d, d.smp[i], k, r));
+  return acc;
+}
+
 struct GradParams {
   int64_t n;
   float* pred;
@@ -102,6 +141,7 @@ struct GradParams {
   const float* weight;
   float* g2w;
   float correct_scale;       // the weight of a correctly classified row is counted as rint(w * correct_scale)
+  DartParams dart;           // DART instantiation only
 };
 
 // expf / logf evaluated in double and rounded once: within the reference's glibc (<1 ulp,
@@ -109,7 +149,9 @@ struct GradParams {
 __device__ __forceinline__ float exp_rn(float x) { return static_cast<float>(exp(static_cast<double>(x))); }
 __device__ __forceinline__ float log_rn(float x) { return static_cast<float>(log(static_cast<double>(x))); }
 
-template <int LOSS, bool WEIGHTED = false>
+// DART: `pred` is the accumulator of the full predictions; the pending tree's update is the DART update of its iteration
+// (its rows' leaf ids are stored in the history), and the gradients are taken at the sampled predictions (p.dart.smp).
+template <int LOSS, bool WEIGHTED = false, bool DART = false>
 __global__ void __launch_bounds__(256) k_pred_grad(GradParams p) {
   double loss = 0;
   unsigned long long correct = 0;
@@ -122,7 +164,13 @@ __global__ void __launch_bounds__(256) k_pred_grad(GradParams p) {
     if (p.pending_tree != nullptr) {
       // UpdatePredictionWithSingleUnivariateTree (loss_utils.cc:214-229): the leaf of a row is its
       // final node id, no traversal needed.
-      pred += p.pending_tree[p.node_of_row[r]].leaf_value;
+      const uint16_t node = p.node_of_row[r];
+      if (DART) {
+        p.dart.hist[static_cast<int64_t>(p.dart.upd_tree) * p.dart.n + r] = node;
+        pred = dart_update(p.dart, pred, p.pending_tree[node].leaf_value, 0, r);
+      } else {
+        pred += p.pending_tree[node].leaf_value;
+      }
       p.pred[r] = pred;
       if (LOSS == 0) {
         // loss_imp_binomial.cc:204-234, float arithmetic as in the reference.
@@ -139,14 +187,15 @@ __global__ void __launch_bounds__(256) k_pred_grad(GradParams p) {
       }
     }
     if (p.compute_grad) {
+      const float at = DART ? dart_sample(p.dart, pred, 0, r) : pred;
       float g, h;
       if (LOSS == 0) {
         const float label = p.label_u8[r] ? 1.f : 0.f;
-        const float proba = 1.f / (1.f + exp_rn(-pred));
+        const float proba = 1.f / (1.f + exp_rn(-at));
         g = label - proba;
         h = proba * (1 - proba);
       } else {
-        g = p.label_f32[r] - pred;
+        g = p.label_f32[r] - at;
         h = 1.f;
       }
       if (WEIGHTED) {

@@ -4,8 +4,8 @@ Same constructor names, meaning and error behaviour as PYDF's
 `ydf.GradientBoostedTreesLearner` (port/python/ydf/learner/specialized_learners_pre_generated.py:
 1847-1930, wrapping GradientBoostedTreesLearner::TrainWithStatusImpl,
 learner/gradient_boosted_trees/gradient_boosted_trees.cc:1154) for the hyper-parameters the hot
-path reads.  Options that select code outside the path (exact splitter, validation split, row
-sampling, DART, other losses ...) raise NotImplementedError instead of being ignored.
+path reads, DART's forest extraction included.  Options that select code outside the path (the
+random categorical splitter, other losses ...) raise NotImplementedError instead of being ignored.
 """
 import os
 import warnings
@@ -69,6 +69,7 @@ class GradientBoostedTreesLearner:
                  num_candidate_attributes: int = -1,
                  num_candidate_attributes_ratio: Optional[float] = None,
                  forest_extraction: str = "MART",
+                 dart_dropout: Optional[float] = None,
                  random_seed: int = 123456,
                  num_threads: Optional[int] = None,
                  sibling_subtraction: bool = True,
@@ -163,8 +164,17 @@ class GradientBoostedTreesLearner:
         self.num_candidate_attributes = int(num_candidate_attributes)
         self.num_candidate_attributes_ratio = (None if num_candidate_attributes_ratio is None
                                                else float(num_candidate_attributes_ratio))
-        if forest_extraction != "MART":
-            raise NotImplementedError("only forest_extraction=MART is implemented")
+        # forest_extraction: MART, or DART (per-iteration dropout of earlier trees, rescaled trees in the model;
+        # ygg_gbt_set_dart, DESIGN.md §24).  dart_dropout None: the reference's default rate, 0.01.
+        if forest_extraction not in ("MART", "DART"):
+            raise NotImplementedError(f"forest_extraction {forest_extraction!r} is not implemented (MART and DART are)")
+        self.forest_extraction = forest_extraction
+        if dart_dropout is not None:
+            if isinstance(dart_dropout, bool) or not isinstance(dart_dropout, (int, float, np.integer, np.floating)):
+                raise TypeError("dart_dropout must be a number or None")
+            if not 0.0 <= float(dart_dropout) <= 1.0:
+                raise ValueError("dart_dropout must be in [0, 1]")
+        self.dart_dropout = 0.01 if dart_dropout is None else float(dart_dropout)
         if task == Task.CLASSIFICATION:
             if loss not in ("DEFAULT", "BINOMIAL_LOG_LIKELIHOOD", "MULTINOMIAL_LOG_LIKELIHOOD"):
                 raise NotImplementedError(f"loss {loss} is outside the accelerated path")
@@ -395,6 +405,8 @@ class GradientBoostedTreesLearner:
             try:
                 if k < train_ds.n_features:
                     gbt.set_candidate_sampling(self.num_candidate_attributes, self.num_candidate_attributes_ratio)
+                if self.forest_extraction == "DART":
+                    gbt.set_dart(self.dart_dropout)
                 if weights is not None:
                     gbt.set_weights(weights)     # before the labels: the initial predictions are weighted
                 gbt.set_labels(labels)
@@ -402,6 +414,13 @@ class GradientBoostedTreesLearner:
                     gbt.set_validation(valid_ds, valid_labels, weights=valid_weights)
                 gbt.train(self.cfg.num_trees)
                 trees = [gbt.get_tree(i) for i in range(gbt.num_trees())]
+                if self.forest_extraction == "DART":
+                    # ScaleRegressorOutput: every leaf of iteration j times w_j, in float (the engine's saved model)
+                    w = gbt.dart_weights()
+                    K = self.cfg.num_classes if self.cfg.loss == _LOSS_ID["MULTINOMIAL_LOG_LIKELIHOOD"] else 1
+                    for i, t in enumerate(trees):
+                        leaf = t["feature"] < 0
+                        t["leaf_value"][leaf] = (t["leaf_value"][leaf].astype(np.float32) * np.float32(w[i // K])).astype(np.float32)
                 category_sets = [gbt.get_category_sets(i, t) for i, t in enumerate(trees)]
                 logs = []
                 for i in range(gbt.num_iterations()):
@@ -421,6 +440,8 @@ class GradientBoostedTreesLearner:
         config = {k: getattr(self.cfg, k) for k, _ in self.cfg._fields_}
         config["num_candidate_attributes"] = self.num_candidate_attributes
         config["num_candidate_attributes_ratio"] = self.num_candidate_attributes_ratio
+        config["forest_extraction"] = self.forest_extraction
+        config["dart_dropout"] = self.dart_dropout if self.forest_extraction == "DART" else None
         model = GradientBoostedTreesModel(spec, trees, init, self.loss, logs, config=config, category_sets=category_sets)
         model.validation_loss, model.early_stopping_triggered = final
         return model
