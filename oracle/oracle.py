@@ -218,6 +218,12 @@ def set_validated_shuffle_mode(mode):
     lib().oracle_set_validated_shuffle_mode(C.c_int32(int(mode)))
 
 
+def set_dart(rate=None):
+    """forest_extraction of gbt_train_validated: DART at this dropout rate (DartPredictionAccumulator,
+    gradient_boosted_trees.cc:3102-3223), or MART for None / a negative rate."""
+    lib().oracle_set_dart(C.c_float(-1.0 if rate is None else float(rate)))
+
+
 def set_hessian_buckets_double(enabled):
     """Cross-check mode: exact (double) hessian-gain buckets instead of the reference's float."""
     lib().oracle_set_hessian_buckets_double(C.c_int32(int(enabled)))
@@ -494,9 +500,19 @@ def gbt_train_validated(bins, num_bins, na_bin, labels, cfg, validation_ratio, n
     if r < 0:
         raise RuntimeError("oracle_gbt_train_validated: node capacity too small")
     k = n_entries.value
-    return dict(in_training=mask.astype(bool), trees=[nodes[offs[i]:offs[i + 1]].copy() for i in range(r)],
-                train_loss=tl[:k], valid_loss=vl[:k], valid_secondary=vs[:k], num_entries=k,
-                validation_loss=fvl.value, early_stopping_triggered=bool(trig.value))
+    out = dict(in_training=mask.astype(bool), trees=[nodes[offs[i]:offs[i + 1]].copy() for i in range(r)],
+               train_loss=tl[:k], valid_loss=vl[:k], valid_secondary=vs[:k], num_entries=k,
+               validation_loss=fvl.value, early_stopping_triggered=bool(trig.value))
+    L = lib()
+    L.oracle_get_dart_num_iterations.restype = C.c_int32
+    n_dart = L.oracle_get_dart_num_iterations()
+    if n_dart > 0:   # DART (set_dart): the trees above are as grown; the model scales iteration j's leaves by dart_weights[j]
+        buf = np.zeros(n_dart, np.int32)
+        out["dart_dropped"] = [buf[:L.oracle_get_dart_dropped(C.c_int32(i), _p(buf, C.c_int32), C.c_int32(n_dart))].tolist()
+                               for i in range(n_dart)]
+        w = np.zeros(n_dart, np.float32)
+        out["dart_weights"] = w[:L.oracle_get_dart_scales(_p(w, C.c_float), C.c_int32(n_dart))].copy()
+    return out
 
 
 LOSS_MULTINOMIAL = 2

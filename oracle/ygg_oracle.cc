@@ -42,6 +42,10 @@
 // held to two properties (unit weights == the pinned unweighted run bit for bit, integer weights == repeated rows).
 // GOSS (SampleTrainingExamplesWithGoss) is pinned on the sampler KAT gradient_boosted_trees_test.cc:472-506; the two
 // golden metric values of the reference's GOSS tests equal its UNSAMPLED Base run's and do not pin the path (DESIGN.md §19).
+// DART (oracle_set_dart: DartPredictionAccumulator's draws, sampled gradients, updates and model scaling in
+// oracle_gbt_train_validated) is pinned on the golden metric values of GradientBoostedTreesOnIris.Dart
+// (gradient_boosted_trees_test.cc:1774-1784: accuracy and log loss within YDF_TEST_METRIC's 1e-4,
+// tests/test_reference_replay.py), on the gbt_iris configuration whose golden run the loop reproduces in full.
 //
 // Every function cites the reference file:line it follows; paths are relative to
 // /root/reference/yggdrasil_decision_forests/.  Storage types are the reference's:
@@ -989,15 +993,22 @@ SplitSearchResult EvalFeature(const Dataset& ds, const TreeConfig& cfg, const ui
 // word, redrawn while >= d + 1 (w = bits of d + 1), and swap.  The reference's golden PYDF models were built against
 // libc++: their tie-breaks between equal-score features follow this order on all 229 ties of three complete runs
 // (tests/test_reference_replay.py).
+// libc++'s uniform_int_distribution over [0, rp) on mt19937: nothing drawn for rp == 1, else the low w bits of one word
+// (2^w >= rp), redrawn while >= rp.
+uint32_t UniformIntLibcxx(uint64_t rp, std::mt19937* g) {
+  if (rp == 1) return 0;
+  int w = 63 - __builtin_clzll(rp);
+  if (rp & ((1ull << w) - 1)) ++w;
+  uint32_t u;
+  do { u = (*g)() & static_cast<uint32_t>((1ull << w) - 1); } while (u >= rp);
+  return u;
+}
+
 void ShuffleLibcxx(std::vector<int32_t>* v, std::mt19937* g) {
   const int64_t n = static_cast<int64_t>(v->size());
   int64_t d = n - 1;
   for (int64_t first = 0; first < n - 1; ++first, --d) {
-    const uint64_t rp = static_cast<uint64_t>(d) + 1;
-    int w = 63 - __builtin_clzll(rp);
-    if (rp & ((1ull << w) - 1)) ++w;
-    uint32_t u;
-    do { u = (*g)() & static_cast<uint32_t>((1ull << w) - 1); } while (u >= rp);
+    const uint32_t u = UniformIntLibcxx(static_cast<uint64_t>(d) + 1, g);
     if (u != 0) std::swap((*v)[first], (*v)[first + u]);
   }
 }
@@ -1586,6 +1597,65 @@ void oracle_mc_loss_w(const int32_t* labels, int32_t K, const float* predictions
 // Candidate-shuffle mode of oracle_gbt_train_validated (0 = dataspec order, 1 = libstdc++, 2 = libc++; FindBestCondition).
 static int g_validated_shuffle_mode = 0;
 
+// forest_extraction = DART in oracle_gbt_train_validated (oracle_set_dart; a negative rate: MART).  The draws and the
+// accumulator restate DartPredictionAccumulator (gradient_boosted_trees.cc:3102-3223) with the standard library that
+// g_validated_shuffle_mode selects (2: libc++, otherwise libstdc++).  The run leaves its dropped sets and the model's
+// per-iteration leaf scales here (oracle_get_dart_*).
+static float g_dart_rate = -1.f;
+static std::vector<std::vector<int32_t>> g_dart_dropped;
+static std::vector<float> g_dart_scales;
+
+// std::uniform_real_distribution<float> on one mt19937 word.  libstdc++'s generate_canonical keeps a result that rounds to
+// 1 just below it; libc++'s returns float(word) / 2^32 as it rounds, 1.0 for the words from 2^32 - 128 on.
+static float DartUnitDraw(std::mt19937* random) {
+  if (g_validated_shuffle_mode == 2) return static_cast<float>((*random)()) / 4294967296.f;
+  return std::uniform_real_distribution<float>()(*random);
+}
+
+// SampleIterIndices (gradient_boosted_trees.cc:3108-3130): nothing drawn before the first iteration; then one unit draw
+// per earlier iteration, dropped iff < rate; an empty set takes one iteration by uniform_int_distribution<int>(0, i - 1).
+static std::vector<int32_t> DartSampleIterIndices(int num_iters, float rate, std::mt19937* random) {
+  std::vector<int32_t> dropped;
+  if (num_iters == 0) return dropped;
+  for (int j = 0; j < num_iters; j++)
+    if (DartUnitDraw(random) < rate) dropped.push_back(j);
+  if (dropped.empty()) {
+    dropped.push_back(g_validated_shuffle_mode == 2 ? static_cast<int32_t>(UniformIntLibcxx(num_iters, random))
+                                                    : std::uniform_int_distribution<int>(0, num_iters - 1)(*random));
+  }
+  return dropped;
+}
+
+// One DartPredictionAccumulator: `acc` the full predictions, per past iteration its trees' leaf of every element
+// (0 + leaf, UpdatePredictions on a zero vector, :3172-3177).  Elements are the loop's predictions, [row][K].
+struct DartAccumulator {
+  std::vector<float>* acc;
+  std::vector<std::vector<float>> per_iter;
+  // GetSampledPredictions (:3141-3163): acc -= p_j * w_j over the dropped iterations in ascending order.
+  void Sampled(const std::vector<int32_t>& dropped, const std::vector<float>& w, int num_threads, std::vector<float>* out) const {
+    *out = *acc;
+    if (dropped.empty()) return;   // GetAllPredictions
+    ParallelFor(num_threads, static_cast<int64_t>(out->size()), 1 << 16, [&](int, int64_t e) {
+      float v = (*out)[e];
+      for (const int32_t j : dropped) v -= per_iter[j][e] * w[j];
+      (*out)[e] = v;
+    });
+  }
+  // UpdateWithNewIteration (:3165-3214) before the weights change: acc += p_new * w_new, then
+  // acc += p_j * w_j * (sf - 1) for each dropped j.
+  void Update(std::vector<float>&& p_new, const std::vector<int32_t>& dropped, const std::vector<float>& w, int num_threads) {
+    const float w_new = 1.0f / (dropped.size() + 1);
+    const float sampled_factor = static_cast<float>(dropped.size()) / (dropped.size() + 1);
+    ParallelFor(num_threads, static_cast<int64_t>(acc->size()), 1 << 16, [&](int, int64_t e) {
+      float v = (*acc)[e];
+      v += p_new[e] * w_new;
+      for (const int32_t j : dropped) v += per_iter[j][e] * w[j] * (sampled_factor - 1.f);
+      (*acc)[e] = v;
+    });
+    per_iter.push_back(std::move(p_new));
+  }
+};
+
 int32_t oracle_gbt_train_validated(const uint16_t* bins, int64_t n_rows, int32_t n_features, const int32_t* num_bins,
                                    const int32_t* na_bin, const int32_t* labels_i32, const float* labels_f32,
                                    const ygg_gbt_config* cfg, float validation_ratio, int32_t num_threads,
@@ -1650,9 +1720,23 @@ int32_t oracle_gbt_train_validated(const uint16_t* bins, int64_t n_rows, int32_t
   int trained = 0;
   const int32_t* vl_i = labels_i32 ? vli.data() : nullptr;
   const float* vl_f = labels_f32 ? vlf.data() : nullptr;
+  // DART (:1311-1324): one accumulator per dataset over pred / vpred, which then hold the full predictions; the two share
+  // the dropped sets and therefore the weights.
+  const bool dart = g_dart_rate >= 0.f;
+  g_dart_dropped.clear();
+  g_dart_scales.clear();
+  DartAccumulator dart_train{&pred, {}}, dart_valid{&vpred, {}};
+  std::vector<float> dart_w, sampled_pred;
   for (int iter = 0; iter < cfg->num_trees; iter++) {
-    if (multinomial) oracle_mc_update_gradients(tl_i, K, pred.data(), NT, g.data(), h.data());
-    else oracle_update_gradients(cfg->loss, tl_i, tl_f, pred.data(), NT, g.data(), h.data());
+    // :1436-1442: the draws come first in the iteration, the gradients are taken at the sampled predictions
+    std::vector<int32_t> dropped;
+    if (dart) {
+      dropped = DartSampleIterIndices(iter, g_dart_rate, &random);
+      dart_train.Sampled(dropped, dart_w, num_threads, &sampled_pred);
+    }
+    const float* grad_pred = dart ? sampled_pred.data() : pred.data();
+    if (multinomial) oracle_mc_update_gradients(tl_i, K, grad_pred, NT, g.data(), h.data());
+    else oracle_update_gradients(cfg->loss, tl_i, tl_f, grad_pred, NT, g.data(), h.data());
     bool sampled;
     if (UsesGoss(*cfg)) {
       if (weighted || multinomial || cfg->use_hessian_gain) return -2;   // not restated
@@ -1675,12 +1759,29 @@ int32_t oracle_gbt_train_validated(const uint16_t* bins, int64_t n_rows, int32_t
     }
     trained = iter + 1;
     if (UsesGoss(*cfg)) g_weights = nullptr;
-    ParallelFor(num_threads, NT, 1 << 16, [&](int, int64_t r) {
-      for (int k = 0; k < K; k++) pred[r * K + k] += LeafOf(ds, new_trees[k], r);
-    });
-    ParallelFor(num_threads, NV, 1 << 16, [&](int, int64_t r) {
-      for (int k = 0; k < K; k++) vpred[r * K + k] += LeafOf(vds, new_trees[k], r);
-    });
+    if (dart) {
+      // :1526-1541: both accumulators take the iteration with the same dropped set, then the dropped weights shrink
+      std::vector<float> p_new(static_cast<size_t>(NT) * K), vp_new(static_cast<size_t>(NV) * K);
+      ParallelFor(num_threads, NT, 1 << 16, [&](int, int64_t r) {
+        for (int k = 0; k < K; k++) p_new[r * K + k] = LeafOf(ds, new_trees[k], r);
+      });
+      ParallelFor(num_threads, NV, 1 << 16, [&](int, int64_t r) {
+        for (int k = 0; k < K; k++) vp_new[r * K + k] = LeafOf(vds, new_trees[k], r);
+      });
+      dart_train.Update(std::move(p_new), dropped, dart_w, num_threads);
+      dart_valid.Update(std::move(vp_new), dropped, dart_w, num_threads);
+      const float sampled_factor = static_cast<float>(dropped.size()) / (dropped.size() + 1);   // :3207-3212
+      for (const int32_t j : dropped) dart_w[j] *= sampled_factor;
+      dart_w.push_back(1.0f / (dropped.size() + 1));
+      g_dart_dropped.push_back(std::move(dropped));
+    } else {
+      ParallelFor(num_threads, NT, 1 << 16, [&](int, int64_t r) {
+        for (int k = 0; k < K; k++) pred[r * K + k] += LeafOf(ds, new_trees[k], r);
+      });
+      ParallelFor(num_threads, NV, 1 << 16, [&](int, int64_t r) {
+        for (int k = 0; k < K; k++) vpred[r * K + k] += LeafOf(vds, new_trees[k], r);
+      });
+    }
     float sec;
     if (multinomial) oracle_mc_loss_w(tl_i, K, pred.data(), train_w, NT, &out_train_loss[iter], &sec);
     else oracle_loss_w(cfg->loss, tl_i, tl_f, pred.data(), train_w, NT, &out_train_loss[iter], &sec);
@@ -1714,6 +1815,11 @@ int32_t oracle_gbt_train_validated(const uint16_t* bins, int64_t n_rows, int32_t
       final_trees = es.best_num_trees;
       *out_early_stopping_triggered = 1;
     }
+  }
+  if (dart) {
+    // :1706-1722, after the truncation: iteration j of the kept ones scales its trees' leaves (ScaleRegressorOutput,
+    // decision_tree.cc:1980-1988) by its weight as the loop ended.  The trees are returned as grown.
+    g_dart_scales.assign(dart_w.begin(), dart_w.begin() + final_trees / K);
   }
   return final_trees;
 }
@@ -1859,6 +1965,23 @@ int32_t oracle_goss_sample(const float* gradient, int64_t n, float alpha, float 
   return static_cast<int32_t>(selected.size());
 }
 void oracle_set_validated_shuffle_mode(int32_t mode) { g_validated_shuffle_mode = mode; }
+// DART in oracle_gbt_train_validated at this dropout rate; negative: off (MART).
+void oracle_set_dart(float rate) { g_dart_rate = rate; }
+// The last DART run: its trained iterations, the dropped set of iteration `iter` (returns its size; -1: capacity too
+// small or no such iteration) and the model's per-iteration leaf scales (returns their number).
+int32_t oracle_get_dart_num_iterations(void) { return static_cast<int32_t>(g_dart_dropped.size()); }
+int32_t oracle_get_dart_dropped(int32_t iter, int32_t* out, int32_t capacity) {
+  if (iter < 0 || iter >= static_cast<int32_t>(g_dart_dropped.size())) return -1;
+  const std::vector<int32_t>& d = g_dart_dropped[iter];
+  if (static_cast<int32_t>(d.size()) > capacity) return -1;
+  std::copy(d.begin(), d.end(), out);
+  return static_cast<int32_t>(d.size());
+}
+int32_t oracle_get_dart_scales(float* out, int32_t capacity) {
+  if (static_cast<int32_t>(g_dart_scales.size()) > capacity) return -1;
+  std::copy(g_dart_scales.begin(), g_dart_scales.end(), out);
+  return static_cast<int32_t>(g_dart_scales.size());
+}
 void oracle_set_hessian_buckets_double(int32_t enabled) { g_hessian_buckets_double = enabled != 0; }
 void oracle_set_stable_category_sort(int32_t mode) { g_stable_category_sort = mode; }
 

@@ -21,6 +21,12 @@ def unit_float(word):
     return min(u, np.nextafter(F32(1), F32(0)))
 
 
+def unit_float_libcxx(word):
+    """libc++'s std::uniform_real_distribution<float> on one mt19937 word: float(word) / 2^32 as rounded, so the words
+    from 2^32 - 128 on give 1.0."""
+    return F32(F32(int(word)) / F32(TWO32))
+
+
 def uniform_int_libstdcxx(next_word, n):
     """libstdc++'s std::uniform_int_distribution<int>(0, n - 1) on a 32-bit engine: Lemire's multiply-shift with rejection
     (one word per try, one word even for n == 1)."""
@@ -48,11 +54,13 @@ def uniform_int_libcxx(next_word, n):
 
 def draw_dropped(next_word, i, rate, libcxx):
     """The dropped set of iteration i: one unit draw per earlier iteration, dropped iff < rate; an empty set takes one
-    iteration drawn uniformly.  `next_word`: the learner's mt19937, one 32-bit word per call."""
+    iteration drawn uniformly.  `next_word`: the learner's mt19937, one 32-bit word per call; `libcxx` selects libc++'s
+    unit draw and uniform integer, else libstdc++'s."""
     if i == 0:
         return []
     rate = F32(rate)
-    dropped = [j for j in range(i) if unit_float(next_word()) < rate]
+    unit = unit_float_libcxx if libcxx else unit_float
+    dropped = [j for j in range(i) if unit(next_word()) < rate]
     if not dropped:
         dropped = [(uniform_int_libcxx if libcxx else uniform_int_libstdcxx)(next_word, i)]
     return dropped

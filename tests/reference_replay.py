@@ -407,13 +407,14 @@ def replay_cxx(ref, data, num_iterations=None, score_rtol=1e-6, leaf_atol=1e-6):
     return seen, np.array(logs)
 
 
-def oracle_loop_cxx(ref, data, stable_category_sort=True, num_threads=1, **config):
+def oracle_loop_cxx(ref, data, stable_category_sort=True, num_threads=1, dart=None, **config):
     """The oracle's WHOLE learner loop on its own state, set up like utils::TrainAndTestTester sets up the reference for a
     C++ test: training fold, C++ dataspec (dictionaries of the model), one thread, libc++ candidate shuffle, default 10 %
     hold-out + early stopping, and — to stand in for the exact numerical splitter — one bucket per distinct value with the
     exact threshold rule (oracle.set_bucket_values).  `config` overrides GBT hyper-parameters; num_threads > 1 selects the
-    concurrent manager (PYDF runs: the model's dictionaries are PYDF's then).  Returns the oracle's result
-    dict plus `predict(columns) -> raw scores` that routes RAW rows by the float thresholds / dictionaries."""
+    concurrent manager (PYDF runs: the model's dictionaries are PYDF's then); `dart` a dropout rate selects DART
+    (oracle.set_dart).  Returns the oracle's result dict plus `predict(columns) -> raw scores` that routes RAW rows by
+    the float thresholds / dictionaries; under DART it sums fl(leaf * w) in tree order, the model's scaled leaves."""
     names = [str(s) for s in ref["column_names"]]
     label = names[int(ref["label_col_idx"])]
     loss = LOSS_OF_MODEL[int(ref["loss"])]
@@ -447,9 +448,11 @@ def oracle_loop_cxx(ref, data, stable_category_sort=True, num_threads=1, **confi
     O.set_validated_shuffle_mode(O.SHUFFLE_LIBCXX)
     O.set_stable_category_sort(stable_category_sort)   # libc++ orders up to 30 equal buckets stably (insertion sort)
     O.set_bucket_values(vals, means)
+    O.set_dart(dart)
     try:
         out = O.gbt_train_validated(np.stack(bins), nb, na, y, cfg, 0.1, num_threads=num_threads, feature_type=ft)
     finally:
+        O.set_dart(None)
         O.set_validated_shuffle_mode(O.SHUFFLE_NONE)
         O.set_stable_category_sort(False)
         O.set_bucket_values(None)
@@ -487,7 +490,10 @@ def oracle_loop_cxx(ref, data, stable_category_sort=True, num_threads=1, **confi
                         x = columns[name][rows].astype(np.float32)
                         go[m] = np.where(np.isnan(x), t["na_value"][nd] != 0, x >= thr[nd])
                 node[act] = np.where(go, t["pos_child"][node[act]], t["neg_child"][node[act]])
-            raw[:, ti % K_out] += t["leaf_value"][node]
+            leaf = t["leaf_value"][node]
+            if dart is not None:
+                leaf = (leaf * out["dart_weights"][ti // K_out]).astype(np.float32)
+            raw[:, ti % K_out] += leaf
         return raw[:, 0] if K_out == 1 else raw
     out["predict"] = predict
     out["labels"] = y

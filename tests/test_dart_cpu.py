@@ -110,3 +110,73 @@ def test_learner_dart_options():
             L("y", forest_extraction="DART", dart_dropout=bad)
     with pytest.raises(NotImplementedError):
         L("y", forest_extraction="RANDOM_FOREST")
+
+
+def _oracle_dart_run(rate, shuffle, K, seed):
+    """A small oracle run (oracle_gbt_train_validated, no hold-out) with DART on; trees of depth 2, so exactly one
+    candidate shuffle per tree, at its root."""
+    from oracle import oracle as O
+    from tests.util import synth_mixed
+    n = 600
+    bins, nb, na, ft, y = synth_mixed(n, 4, [6, 40], seed=seed, task="binary")
+    if K > 1:
+        y = ((bins[0].astype(np.int64) + bins[1]) % K + 1).astype(np.int32)
+        y = np.where(np.random.default_rng(seed).random(n) < 0.3, (y % K) + 1, y).astype(np.int32)
+    cfg = O.default_config(loss=O.LOSS_MULTINOMIAL if K > 1 else O.LOSS_BINOMIAL, num_classes=K if K > 1 else 0,
+                           num_trees=30, max_depth=2, shrinkage=0.3, random_seed=seed)
+    O.set_validated_shuffle_mode(shuffle)
+    O.set_dart(rate)
+    try:
+        out = O.gbt_train_validated(bins, nb, na, y, cfg, 0.0, num_threads=1, feature_type=ft)
+    finally:
+        O.set_dart(None)
+        O.set_validated_shuffle_mode(O.SHUFFLE_NONE)
+    return out, bins.shape[0], int(cfg.random_seed)
+
+
+@pytest.mark.parametrize("K", [1, 3])
+@pytest.mark.parametrize("shuffle", ["libstdcxx", "libcxx"])
+@pytest.mark.parametrize("rate", [0.0, 0.1, 0.5, 1.0])
+def test_oracle_dart_draws_match_the_restatement(rate, shuffle, K):
+    """The oracle's DART loop (oracle.set_dart) and tests/dart_ref.py are two restatements of the reference's draws: on the
+    same seed the oracle's dropped sets equal dart_ref.draw_dropped replayed on the learner's mt19937 (its words taken in
+    the loop's order: the iteration's draws, then one candidate shuffle per tree), and its weights equal
+    dart_ref.weights_after of those sets."""
+    from oracle import oracle as O
+    mode = O.SHUFFLE_LIBCXX if shuffle == "libcxx" else O.SHUFFLE_LIBSTDCXX
+    out, F, seed = _oracle_dart_run(rate, mode, K, seed=17 + K)
+    iters = out["num_entries"]
+    assert iters == 30 and len(out["trees"]) == 30 * K and len(out["dart_dropped"]) == iters
+    rng = O.Rng(seed)
+    for i in range(iters):
+        want = D.draw_dropped(rng.next, i, rate, libcxx=shuffle == "libcxx")
+        assert out["dart_dropped"][i] == want, (i, out["dart_dropped"][i], want)
+        for t in out["trees"][i * K:(i + 1) * K]:
+            assert t["depth"].max() <= 2   # the root is the tree's only node that searches a split
+            if shuffle == "libcxx":
+                rng.shuffle_libcxx(F)
+            else:
+                rng.shuffle(F)
+    assert np.array_equal(out["dart_weights"], D.weights_after(out["dart_dropped"]))
+    if rate == 1.0:
+        assert all(d == list(range(i)) for i, d in enumerate(out["dart_dropped"]))
+    if rate == 0.0:
+        assert all(len(d) == 1 for d in out["dart_dropped"][1:])
+
+
+def test_oracle_without_dart_is_unchanged_by_an_earlier_dart_run():
+    """set_dart(None) restores MART: the same run before and after a DART run gives the same trees and losses, and no
+    DART state."""
+    from oracle import oracle as O
+    from tests.util import synth_mixed
+    bins, nb, na, ft, y = synth_mixed(800, 4, [6, 40], seed=3, task="binary")
+    cfg = O.default_config(loss=O.LOSS_BINOMIAL, num_trees=12, max_depth=4, shrinkage=0.3)
+    before = O.gbt_train_validated(bins, nb, na, y, cfg, 0.2, num_threads=1, feature_type=ft)
+    _oracle_dart_run(0.5, O.SHUFFLE_LIBCXX, 1, seed=5)
+    after = O.gbt_train_validated(bins, nb, na, y, cfg, 0.2, num_threads=1, feature_type=ft)
+    assert "dart_dropped" not in after and "dart_weights" not in after
+    assert np.array_equal(before["train_loss"], after["train_loss"])
+    assert np.array_equal(before["valid_loss"], after["valid_loss"])
+    assert len(before["trees"]) == len(after["trees"])
+    for a, b in zip(before["trees"], after["trees"]):
+        assert np.array_equal(a, b)

@@ -379,6 +379,29 @@ def test_oracle_training_loop_reproduces_the_multinomial_runs():
         assert abs(out["validation_loss"] - float(ref["validation_loss"])) <= tol, name
 
 
+def test_oracle_dart_loop_reproduces_the_golden_metrics_of_the_iris_dart_test():
+    """GradientBoostedTreesOnIris.Dart (gradient_boosted_trees_test.cc:1774-1784): the gbt_iris configuration (the tester's
+    training fold, one thread, libc++ shuffle, 10 % hold-out, early stopping) with forest_extraction DART at dropout 0.1,
+    100 trees and the DART default shrinkage 1.0 (:3257-3262).  num_candidate_attributes 8 samples nothing on Iris's 4
+    features.  The oracle's DART loop (oracle.set_dart) gives the golden accuracy 0.9733 and log loss 0.2019 on the test
+    fold within YDF_TEST_METRIC's 1e-4: the draws, the sampled gradients, the early stopping and the scaled model follow
+    the reference."""
+    ref, data = R.load_run("cxx_iris")
+    z = np.load(os.path.join(R.G, "dart_cxx_test_folds.npz"))
+    names = [str(s) for s in ref["column_names"]]
+    assert all(np.array_equal(z[f"iris_train_{n}"], data[n]) for n in names)   # the golden run's rows are the DART run's
+    test = {n: z[f"iris_test_{n}"] for n in names}
+    out = R.oracle_loop_cxx(ref, data, stable_category_sort=3, num_trees=100, shrinkage=1.0, dart=0.1)
+    assert out["num_entries"] == len(out["dart_dropped"]) and len(out["dart_weights"]) == len(out["trees"]) // 3
+    voc = [str(s) for s in ref["vocabulary_class"]]
+    yt = np.array([voc.index(str(s)) for s in test["class"]])
+    raw = out["predict"](test).astype(np.float64)
+    e = np.exp(raw - raw.max(1, keepdims=True))
+    p = e / e.sum(1, keepdims=True)
+    assert abs(float(np.mean(p.argmax(1) + 1 == yt)) - 0.9733) < 1e-4
+    assert abs(float(-np.mean(np.log(p[np.arange(len(yt)), yt - 1]))) - 0.2019) < 1e-4
+
+
 @pytest.mark.parametrize("test_name,config,golden", [
     ("FakeMulticlass (:1315-1331)", dict(), (0.8646, 0.2966)),
     ("FakeMulticlassL2Regularization (:1335-1351)", dict(l2_regularization=0.1), (0.8725, 0.2953)),

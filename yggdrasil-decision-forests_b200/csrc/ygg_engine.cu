@@ -2122,9 +2122,13 @@ int draw_dart(ygg_gbt* h) {
   const int i = h->iters_done;
   std::vector<int32_t> dropped;
   if (i > 0) {
+    // libc++'s uniform_real_distribution<float> is float(word) / 2^32 as rounded, 1.0 for the words from 2^32 - 128 on;
+    // libstdc++'s keeps those just below 1.  The two differ at rate 1 only.
     std::uniform_real_distribution<float> unif_dist_unit;
-    for (int j = 0; j < i; j++)
-      if (unif_dist_unit(h->tie_rng) < h->dart_rate) dropped.push_back(j);
+    for (int j = 0; j < i; j++) {
+      const float u = h->cfg.candidate_shuffle == 2 ? static_cast<float>(h->tie_rng()) / 4294967296.f : unif_dist_unit(h->tie_rng);
+      if (u < h->dart_rate) dropped.push_back(j);
+    }
     if (dropped.empty())
       dropped.push_back(h->cfg.candidate_shuffle == 2 ? static_cast<int32_t>(uniform_int_libcxx(static_cast<uint64_t>(i), &h->tie_rng))
                                                       : std::uniform_int_distribution<int>(0, i - 1)(h->tie_rng));
