@@ -235,7 +235,8 @@ int ygg_gbt_create(ygg_gbt** out, ygg_dataset* ds, const ygg_gbt_config* cfg);
 int ygg_gbt_destroy(ygg_gbt* h);
 
 /* Labels.  i32: integerised categorical label as the reference stores it (1 = negative,
- * 2 = positive; loss_imp_binomial.cc:133).  f32: regression target. */
+ * 2 = positive; loss_imp_binomial.cc:133).  f32: regression target.  INVALID_ARGUMENT after ygg_gbt_set_row_shard*: a
+ * row shard holds the job's initial prediction, which this rank's labels would replace. */
 int ygg_gbt_set_labels_i32(ygg_gbt* h, const int32_t* labels, int64_t n);
 int ygg_gbt_set_labels_f32(ygg_gbt* h, const float* labels, int64_t n);
 
@@ -259,7 +260,9 @@ int ygg_gbt_set_weights_f32(ygg_gbt* h, const float* weights, int64_t n);
  * gathers the two row sets on the device, ygg_gbt_set_validation_* attaches the held-out rows (same
  * features and binning as the training dataset).  ygg_gbt_train then applies cfg.early_stopping;
  * afterwards ygg_gbt_num_trees is the truncated model size and ygg_gbt_num_iterations the number of
- * iterations that have log entries (training stopped there).  Not combined with sharding. */
+ * iterations that have log entries (training stopped there).  Not combined with sharding: YGG_ERR_UNIMPLEMENTED in
+ * either call order (ygg_gbt_set_validation_* on a sharded handle, or a shard setter with world > 1 on a handle with
+ * validation rows), since every rank would evaluate and stop on its own. */
 int ygg_validation_split_mask(uint32_t random_seed, int64_t n_rows, float validation_ratio,
                               uint8_t* out_in_training /* [n_rows] 1 = training row */);
 int ygg_dataset_split_rows(const ygg_dataset* ds, const uint8_t* select, ygg_dataset** selected,
@@ -282,7 +285,9 @@ int ygg_gbt_final_validation(ygg_gbt* h, float* validation_loss, int32_t* early_
  * features [feature_begin, feature_end) only; all ranks hold all columns so the row partition
  * is local.  `exchange` is called once per tree level with this rank's packed best-split
  * records (device pointer, `bytes` bytes) and must all-gather them into `recv` (device pointer,
- * world*bytes) on `stream` (a cudaStream_t) — NCCL in production, see INTEGRATION.md. */
+ * world*bytes) on `stream` (a cudaStream_t) — NCCL in production, see INTEGRATION.md.
+ * Refused up front: wide and presorted columns, candidate feature sampling, DART, candidate_shuffle and (world > 1)
+ * validation rows; the multinomial loss, subsample < 1 and GOSS by the first ygg_gbt_step, before any collective. */
 typedef int (*ygg_allgather_fn)(void* ctx, const void* send, void* recv, int64_t bytes,
                                 void* stream);
 int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature_end,
@@ -294,8 +299,13 @@ int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature
  * exact and independent of the reduction order, so trees are identical for any world size.  Child
  * statistics ride in the same buffer.  `allreduce(ctx, buf, count, dtype, op, stream)` must reduce
  * `count` elements in place on `stream`: dtype 0 = u32, 1 = u64, 2 = f64; op 0 = sum, 1 = max.
- * Call after ygg_gbt_set_labels_*; `initial_prediction` is the job-wide value (the harness owns
- * the global label statistics, loss_imp_binomial.cc:65-99). */
+ * Call after ygg_gbt_set_labels_* (labels set afterwards are refused); `initial_prediction` is the job-wide value (the
+ * harness owns the global label statistics, loss_imp_binomial.cc:65-99).  Every rank holds at least one row:
+ * ygg_dataset_create refuses an empty dataset with INVALID_ARGUMENT, so a rank without rows is refused before it has a
+ * handle or calls a collective; give each rank at least one row, or use fewer ranks.  Ranks may hold any other
+ * uneven share, down to one row.  Refused up front, before any collective, like the feature shard: wide and presorted
+ * columns, candidate feature sampling, DART, candidate_shuffle and validation rows.  The multinomial loss, subsample < 1
+ * and GOSS are refused (YGG_ERR_UNIMPLEMENTED) by the first ygg_gbt_step, before that iteration's first collective. */
 typedef int (*ygg_allreduce_fn)(void* ctx, void* buf, int64_t count, int32_t dtype, int32_t op, void* stream);
 int ygg_gbt_set_row_shard(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_rows_global,
                           float initial_prediction, ygg_allreduce_fn allreduce, void* ctx);
@@ -306,7 +316,8 @@ int ygg_gbt_set_row_shard(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_row
  * chunk and the best splits are all-gathered like in feature sharding (<= 3.5 KB): half the collective
  * bytes of the all-reduce and no replicated scan.  `reducescatter(ctx, buf, count_per_rank, dtype, op,
  * stream)` reduces world*count_per_rank elements in place, rank r's result at buf + r*count_per_rank;
- * `allreduce` is still used for a few scalars per iteration. */
+ * `allreduce` is still used for a few scalars per iteration.  INVALID_ARGUMENT, before any collective, when
+ * world > num_features or the features do not cut into `world` non-empty chunks ((world - 1) * c >= F). */
 typedef int (*ygg_reducescatter_fn)(void* ctx, void* buf, int64_t count_per_rank, int32_t dtype, int32_t op,
                                     void* stream);
 int ygg_gbt_set_row_shard_scatter(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_rows_global,

@@ -2877,10 +2877,20 @@ static int set_initial_predictions(ygg_gbt* h) {
   return YGG_OK;
 }
 
+// A row shard took the job's initial prediction from the caller and filled the predictions with it; new labels would
+// replace it with this rank's own and restart the iteration count, and the rank would train apart from the others
+// (tests/test_gpu_shard_exact.py::test_labels_after_a_row_shard_are_refused).
+static int refuse_labels_after_row_shard(const ygg_gbt* h) {
+  if (h->shard_mode == kShardRows)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "labels after the row shard: set the labels first, then ygg_gbt_set_row_shard*");
+  return YGG_OK;
+}
+
 int ygg_gbt_set_labels_i32(ygg_gbt* h, const int32_t* labels, int64_t n) {
   if (!h || !labels) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (n != h->ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "label count %lld != rows %lld", static_cast<long long>(n), static_cast<long long>(h->ds->n));
   if (!is_logit(h)) return set_error(YGG_ERR_INVALID_ARGUMENT, "integer labels need a log-likelihood loss");
+  YGG_RETURN_IF_ERROR(refuse_labels_after_row_shard(h));
   YGG_CUDA(cudaSetDevice(h->ds->device));
   if (is_multinomial(h)) {
     std::vector<uint8_t> cls(n);
@@ -2946,6 +2956,7 @@ int ygg_gbt_set_labels_f32(ygg_gbt* h, const float* labels, int64_t n) {
   if (!h || !labels) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (n != h->ds->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "label count %lld != rows %lld", static_cast<long long>(n), static_cast<long long>(h->ds->n));
   if (h->cfg.loss != YGG_LOSS_SQUARED_ERROR) return set_error(YGG_ERR_INVALID_ARGUMENT, "float labels need the squared-error loss");
+  YGG_RETURN_IF_ERROR(refuse_labels_after_row_shard(h));
   YGG_CUDA(cudaSetDevice(h->ds->device));
   // MeanSquaredErrorLoss::InitialPredictions (loss_imp_mean_square_error.cc:56-88).
   double s = 0;
@@ -3042,6 +3053,15 @@ int ygg_gbt_set_validation_weights_f32(ygg_gbt* h, const float* weights, int64_t
   return YGG_OK;
 }
 
+// Validation rows are evaluated on one rank's handle, unreduced: every rank would compute its own loss and early-stopping
+// decision, and ranks that stop at different iterations leave a collective unmatched.  attach_validation refuses them on
+// a sharded handle; the shard setters refuse a handle that already has them
+// (tests/test_gpu_shard_exact.py::test_validation_with_a_shard_is_refused).
+static int refuse_validation_with_shard(const ygg_gbt* h, int32_t world) {
+  if (world > 1 && h->vds != nullptr) return set_error(YGG_ERR_UNIMPLEMENTED, "validation rows are not combined with sharding");
+  return YGG_OK;
+}
+
 int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature_end, int32_t rank,
                               int32_t world, ygg_allgather_fn exchange, void* ctx) {
   if (!h) return set_error(YGG_ERR_INVALID_ARGUMENT, "null handle");
@@ -3055,6 +3075,7 @@ int ygg_gbt_set_feature_shard(ygg_gbt* h, int32_t feature_begin, int32_t feature
   if (world > 1 && h->cfg.candidate_shuffle != 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate_shuffle is not combined with sharding");
   if (h->sample_k_valid > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate feature sampling is not combined with sharding");
   if (h->dart) return set_error(YGG_ERR_UNIMPLEMENTED, "DART is not combined with sharding");
+  YGG_RETURN_IF_ERROR(refuse_validation_with_shard(h, world));
   YGG_CUDA(cudaSetDevice(h->ds->device));
   h->f_begin = feature_begin; h->f_end = feature_end; h->rank = rank; h->world = world;
   h->hist_f_begin = feature_begin; h->hist_f_end = feature_end;
@@ -3082,6 +3103,7 @@ int ygg_gbt_set_row_shard(ygg_gbt* h, int32_t rank, int32_t world, int64_t n_row
   if (h->sample_k_valid > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "candidate feature sampling is not combined with sharding");
   if (h->dart) return set_error(YGG_ERR_UNIMPLEMENTED, "DART is not combined with sharding");
   if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "shard must be set before training");
+  YGG_RETURN_IF_ERROR(refuse_validation_with_shard(h, world));
   YGG_CUDA(cudaSetDevice(h->ds->device));
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
   h->rank = rank; h->world = world;
@@ -3117,12 +3139,14 @@ int ygg_gbt_set_row_shard_scatter(ygg_gbt* h, int32_t rank, int32_t world, int64
   if (h->ds->n_num() > 0) return set_error(YGG_ERR_UNIMPLEMENTED, "presorted numerical columns (ygg_dataset_set_numerical_column) are single GPU: not combined with row shards");
   if (world > 1 && (!reducescatter || !allgather)) return set_error(YGG_ERR_INVALID_ARGUMENT, "world > 1 needs reduce-scatter and all-gather functions");
   if (world > h->ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "more ranks (%d) than features (%d)", world, h->ds->F);
+  // histograms cover every feature; the scan / best-split search covers this rank's chunk of them.  Checked before the
+  // row shard, whose weight scales are all-reduced: a refusal after that collective would leave the handle half sharded
+  // (tests/test_gpu_shard_exact.py::test_scatter_chunks_refused_before_any_collective).
+  const int f_chunk = (h->ds->F + world - 1) / world;
+  if (world > 1 && static_cast<int64_t>(world - 1) * f_chunk >= h->ds->F)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "%d features do not split into %d non-empty chunks of %d", h->ds->F, world, f_chunk);
   YGG_RETURN_IF_ERROR(ygg_gbt_set_row_shard(h, rank, world, n_rows_global, initial_prediction, allreduce, ctx));
   if (world <= 1) return YGG_OK;
-  // histograms cover every feature; the scan / best-split search covers this rank's chunk of them
-  const int f_chunk = (h->ds->F + world - 1) / world;
-  if (static_cast<int64_t>(world - 1) * f_chunk >= h->ds->F)
-    return set_error(YGG_ERR_INVALID_ARGUMENT, "%d features do not split into %d non-empty chunks of %d", h->ds->F, world, f_chunk);
   h->scatter = true;
   h->reducescatter = reducescatter;
   h->exchange = allgather;
