@@ -313,25 +313,39 @@ __global__ void __launch_bounds__(kSegThreads, kSegMinBlocks) k_hist_seg(SegPara
     }
     __syncthreads();
 
-    // flush the non-empty bins of the group's features and zero every touched word for the next item.  A column of the
-    // shard receives <= 8191 updates, so its count is 0 only when both its words are; the others (re-read features,
-    // FPL = 2: the shard's neighbours and the row's zero padding) may receive any number and are always cleared.
-    for (int i = tid; i < kMaxBins * FI; i += kSegThreads) {
-      const int bin = i / FI, k = i - bin * FI;        // k = half * FL + lane
-      const int f = f0 + (k % FL) * FPL + k / FL;      // its shard feature
-      const bool in = f >= 0 && f < p.f_count;
-      uint32_t* w = s_bins + bin * 2 * FI + k;
-      const uint32_t c = w[0];
-      if (c == 0u && in) continue;
-      const uint32_t lo32 = w[FI];
-      w[0] = 0u;
-      w[FI] = 0u;
-      if (!in) continue;
-      size_t oc;
-      const size_t o = slot_hist_offset(slot, f, bin, p.f_chunk, p.chunk_stride, &oc);
-      const unsigned long long base = static_cast<unsigned long long>(c >> kPackedCntBits) << kPackedCoarseShift;
-      atomicAdd(&p.hist_sum[o], base + static_cast<uint32_t>(lo32 - static_cast<uint32_t>(base)));
-      atomicAdd(&p.hist_cnt[oc], c & kPackedMaxUpdates);
+    // flush the non-empty bins of the group's features and zero every word for the next item.  A column of the shard
+    // receives <= 8191 updates, so its count is 0 only when both its words are; the others (re-read features, FPL = 2:
+    // the shard's neighbours and the row's zero padding) may receive any number and are cleared, never flushed.
+    // The global planes are [slot][feature][bin]: a warp instruction whose lanes hold TB consecutive bins of each of QL
+    // features reduces into QL x 2 sectors of sums and QL x 1 of counts (TB = 8), where one lane per feature (the
+    // shared layout's order) touched 32 sectors of each.  Lane (r, q) takes bin r of a tile of TB bins and the 4 adjacent
+    // columns 4q..4q+3 (one half of a lane pair, FL % 4 == 0) of both planes with two 16-byte loads: the 8 lanes of a
+    // quarter-warp (one 16-byte access phase) cover 8 / QL bins x 4 QL columns, a 2-way bank conflict.
+    constexpr int QL = FI >= 16 ? 4 : 2;                // column quads per tile
+    constexpr int TB = 32 / QL;                         // bins per tile
+    constexpr int kQuadGroups = FI / (4 * QL);
+    constexpr int kTiles = kMaxBins / TB * kQuadGroups;
+    const int tr = lane / QL, tq = lane % QL;
+    for (int t = warp; t < kTiles; t += kWarps) {
+      const int bin = t / kQuadGroups * TB + tr;
+      const int k0 = (t % kQuadGroups * QL + tq) * 4;  // k = half * FL + lane
+      uint4* w = reinterpret_cast<uint4*>(s_bins + bin * 2 * FI + k0);
+      const uint4 c4 = w[0], l4 = w[FI / 4];
+      w[0] = make_uint4(0u, 0u, 0u, 0u);
+      w[FI / 4] = make_uint4(0u, 0u, 0u, 0u);
+      const uint32_t cs[4] = {c4.x, c4.y, c4.z, c4.w}, ls[4] = {l4.x, l4.y, l4.z, l4.w};
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int k = k0 + j;
+        const int f = f0 + (k % FL) * FPL + k / FL;   // its shard feature
+        const uint32_t c = cs[j];
+        if (c == 0u || f < 0 || f >= p.f_count) continue;
+        size_t oc;
+        const size_t o = slot_hist_offset(slot, f, bin, p.f_chunk, p.chunk_stride, &oc);
+        const unsigned long long base = static_cast<unsigned long long>(c >> kPackedCntBits) << kPackedCoarseShift;
+        atomicAdd(&p.hist_sum[o], base + static_cast<uint32_t>(ls[j] - static_cast<uint32_t>(base)));
+        atomicAdd(&p.hist_cnt[oc], c & kPackedMaxUpdates);
+      }
     }
   }
 }
