@@ -364,6 +364,28 @@ def test_large_table_deepest_tree():
     assert e.value.code == 4 and "8-bit slots" in str(e.value)
 
 
+def test_gradient_sum_of_a_node_above_2_to_the_23_rows():
+    """k_node_stats removes the 2^30 bias of every row's 31-bit gradient code in integers: over more than 2^23 rows the
+    biased sum passes 2^53, where a double holds only even integers.  The root of 2^23 + 8192 rows with every gradient 0
+    but one of 1.0 (P = 1, code 2^30) and one of 2^-30 (code 1): an odd biased sum, stat[0] = 1 + 2^-30 exactly; a
+    rounded conversion gives 1 or 1 + 2^-29."""
+    n = 2 ** 23 + 8192
+    bins = np.zeros((1, n), np.uint8)
+    bins[0, n // 2:] = 1
+    ds = ydf_b200.Dataset(bins, np.array([2], np.int32), np.zeros(1, np.int32))
+    cfg = ydf_b200.default_config(loss=1, max_depth=2, min_examples=1)
+    gbt = ydf_b200.Gbt(ds, cfg)
+    gbt.set_labels(np.zeros(n, F32))
+    g = np.zeros(n, F32)
+    g[0], g[n - 1] = 1.0, 2.0 ** -30
+    tree = gbt.train_tree_on_gradients(g)
+    assert tree[0]["num_examples"] == n
+    assert tree[0]["stat"][0] == 1.0 + 2.0 ** -30, repr(tree[0]["stat"][0])
+    assert tree[0]["leaf_value"] == R.leaf_value(1.0 + 2.0 ** -30, float(n), cfg, False)
+    gbt.close()
+    ds.close()
+
+
 def test_weighted_near_pure_split_score():
     """Example weights, squared error, 300K rows: two regions of constant label, one of them split into halves whose
     labels differ by two units of the 24-bit gradient code (2 P / 2^23), about the least difference whose weighted score

@@ -42,12 +42,14 @@ def same_f32(a, b):
     return (np.isnan(a) and np.isnan(b)) or a == b
 
 
-def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1, sel=None, select=None):
+def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1, sel=None, select=None, hist_of=None):
     """Compares every captured candidate of the tree with the reference; -> number of (node, feature) pairs checked.
     `cols`: per feature (kind, codes or stored values, buckets, bucket values), kind 'num' / 'cat' (byte), 'wide_num' /
     'wide_cat' (uint16), 'pre' (presorted).  `w`: example weights (the rows then carry w*g in `g`).  `sel`: the rows the
     tree was trained on (subsample / GOSS; None: all).  `select(level, j, cap)`: the feature node j of the level must
-    split on (-1: none), in place of the first maximum in feature order (candidate sampling)."""
+    split on (-1: none), in place of the first maximum in feature order (candidate sampling).  `hist_of(level, cap,
+    rows_of, q, hq)`: the level's bucket sums in one pass (tests/level_hist_ref.LevelHist), a function (j, f) -> (cnt,
+    s, hs) or None (then, and without a provider, scan_ref.bucket_sums per node and feature)."""
     wide = list(getattr(gbt.dataset, "wide", {}))
     sets = gbt.get_category_sets(tree_index, tree) if any(c[0] == "wide_cat" for c in cols) else {}
     rows_of = route(tree, cols, sets)
@@ -73,6 +75,7 @@ def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1, sel=None, sele
         if level == 0 or not cfg.sibling_subtraction:
             assert not cap["derived"].any(), f"level {level}: derived nodes"
         derived_seen += int(cap["derived"].sum())
+        level_sums = hist_of(level, cap, rows_of, q, hq) if hist_of is not None else None
         for j in range(len(cap["node"])):
             pre = int(cap["node"][j])
             rows = rows_of[pre]
@@ -86,7 +89,8 @@ def check_scan(gbt, cfg, tree, cols, g, h, w=None, tree_index=-1, sel=None, sele
                     B = len(distinct)
                     cnt, s, hs = S.bucket_sums(inv, np.arange(len(rows)), q[rows], hq[rows], B)
                 else:
-                    cnt, s, hs = S.bucket_sums(codes, rows, q, hq, B)
+                    sums = level_sums(j, f) if level_sums is not None else None
+                    cnt, s, hs = sums if sums is not None else S.bucket_sums(codes, rows, q, hq, B)
                 cat = kind in ("cat", "wide_cat")
                 l2 = cfg.l2_regularization_categorical if cat else cfg.l2_regularization
                 order = np.arange(B)

@@ -271,6 +271,11 @@ __device__ __forceinline__ uint32_t quant_stat_signed(float v, float scale) {   
 __device__ __forceinline__ uint32_t quant_stat_unsigned(float v, float scale) {  // v >= 0 -> [0, 2^31]
   return min(__float2uint_rn(v * scale), 0x80000000u);  // v == its power-of-two cover stays exact
 }
+// A node's unbiased gradient-code sum from its biased 31-bit sum over n rows, as a double.  The bias is removed in integers
+// first: the biased sum of a node of more than 2^23 rows passes 2^53, where a double no longer holds every integer.
+__device__ __forceinline__ double unbiased_sg(unsigned long long sg, int64_t n) {
+  return static_cast<double>(static_cast<long long>(sg) - static_cast<long long>(n) * static_cast<long long>(kSBias));
+}
 
 __global__ void __launch_bounds__(256) k_quantize(QuantParams p) {
   const float P = p.fixed_g_pow2 > 0.f ? p.fixed_g_pow2 : pow2_cover(p.st->gmax_bits);
@@ -1585,8 +1590,8 @@ __global__ void k_node_stats(StatsParams p) {
         const unsigned long long sg_n = pos_smaller ? par.sg - nd.sg : ss[0];
         const unsigned long long sh_n = pos_smaller ? par.sh - nd.sh : ss[1];
         const double np_ = n, nn_ = static_cast<double>(sib.n);
-        const double Sp = (static_cast<double>(static_cast<long long>(nd.sg)) - np_ * static_cast<double>(kSBias)) * ginv;
-        const double Sn = (static_cast<double>(static_cast<long long>(sg_n)) - nn_ * static_cast<double>(kSBias)) * ginv;
+        const double Sp = unbiased_sg(nd.sg, nd.n) * ginv;
+        const double Sn = unbiased_sg(sg_n, sib.n) * ginv;
         double score;
         if (!p.use_hessian) {
           // exact numerator, as in boundary_score: the biases cancel, d = (sg_pos*n_neg - sg_neg*n_pos) * ginv
@@ -1609,7 +1614,7 @@ __global__ void k_node_stats(StatsParams p) {
         if (score > 0.0) par.score = static_cast<float>(score);
       }
     }
-    const double sum_g = (static_cast<double>(static_cast<long long>(nd.sg)) - n * static_cast<double>(kSBias)) * ginv;
+    const double sum_g = unbiased_sg(nd.sg, nd.n) * ginv;
     double sum_h = p.has_h ? static_cast<double>(nd.sh) * hinv : n;
     const double sum_g2 = static_cast<double>(nd.sg2) * g2inv;
     if (sum_h <= kMinHessianForNewtonStep) sum_h = kMinHessianForNewtonStep;
@@ -1734,8 +1739,8 @@ __global__ void __launch_bounds__(1024) k_weight_sums_finish(WeightSumParams p) 
         const NodeRec& pc = p.nodes[nd.pos_child];
         const NodeRec& nc = p.nodes[nd.neg_child];
         const double ginv = static_cast<double>(p.st->g_pow2) / static_cast<double>(1u << (kSBits - 1));
-        const double Sp = (static_cast<double>(static_cast<long long>(pc.sg)) - static_cast<double>(pc.n) * static_cast<double>(kSBias)) * ginv;
-        const double Sn = (static_cast<double>(static_cast<long long>(nc.sg)) - static_cast<double>(nc.n) * static_cast<double>(kSBias)) * ginv;
+        const double Sp = unbiased_sg(pc.sg, pc.n) * ginv;
+        const double Sn = unbiased_sg(nc.sg, nc.n) * ginv;
         const double Wp = static_cast<double>(x[0]) * winv, Wn = static_cast<double>(y[0]) * winv;
         if (Wp > 0.0 && Wn > 0.0) {
           const double W0 = Wp + Wn;
