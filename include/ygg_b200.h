@@ -465,18 +465,24 @@ int ygg_tree_train_on_gradients(ygg_gbt* h, const float* gradients, const float*
 /* Level-histogram seam (FillExampleBucketSet, learner/decision_tree/splitter_scanner.h:859-909): the histogram phase of
  * one tree level, run by the same code as training, on caller-chosen gradients and slots. */
 enum ygg_hist_mode {
-  YGG_HIST_ROOT_SUM = 0,  /* k_hist, root layout: no count atomics, counts from the precomputed root count histogram */
+  YGG_HIST_ROOT_SUM = 0,  /* root layout: no count atomics, counts from the precomputed root count histogram; k_hist, or
+                             k_hist_root_rows (root_lanes = 32) */
   YGG_HIST_PACKED = 1,    /* k_hist, packed count | coarse-sum words (no bin may take more than 8191 rows per work item) */
   YGG_HIST_SHARED = 2,    /* k_hist, count | carries words (any data; the only layout with a second plane) */
   YGG_HIST_HIST2 = 3,     /* k_hist2: its root variant at level 0, its packed variant below */
   YGG_HIST_SEGMENTED = 4, /* k_hist_seg: packed words, one slot per work item, rows gathered from a row-major copy (level >= 1) */
 };
-typedef struct ygg_hist_plan {  /* one level's k_hist / k_hist2 / k_hist_seg launch */
+typedef struct ygg_hist_plan {  /* one level's k_hist / k_hist2 / k_hist_seg / k_hist_root_rows launch */
   int32_t mode;            /* enum ygg_hist_mode */
   int32_t group;           /* features per work item G (k_hist, 1..8), or feature lanes FL (k_hist2, k_hist_seg: 8, 16, 32;
-                              k_hist_seg at 32 lanes over more than 32 features takes two adjacent features per lane) */
-  int32_t hist2_tiles;     /* sub-tiles of 1024 rows per tile T (k_hist2 only: 1, 2) */
-  int32_t chunk_blocks;    /* 8192-row blocks per work item, 1..127 */
+                              k_hist_seg at 32 lanes over more than 32 features takes two adjacent features per lane), or
+                              features per lane (k_hist_root_rows: 4) */
+  union {                  /* by mode (the struct keeps its 24 bytes) */
+    int32_t hist2_tiles;   /* YGG_HIST_HIST2: sub-tiles of 1024 rows per tile T (1, 2) */
+    int32_t root_lanes;    /* YGG_HIST_ROOT_SUM: 0 = k_hist (G in `group`), 32 = k_hist_root_rows (lanes = features of
+                              the row-major copy, chunk_blocks 1..2048) */
+  };
+  int32_t chunk_blocks;    /* 8192-row blocks per work item, 1..127 (k_hist_root_rows: 1..2048) */
   int32_t slot_window;     /* 0: one pass over every slot; else slots per pass (multi-pass k_hist + one dummy slot) */
   int32_t grid;            /* CTAs */
 } ygg_hist_plan;
@@ -492,7 +498,8 @@ int ygg_debug_hist_plan(const ygg_gbt* h, int32_t level, ygg_hist_plan* out);
  * out_second the raw sums of the second plane (NULL without one); out_scales = {P, V} (V = 0 without a second plane).
  * Refuses (INVALID_ARGUMENT, before any launch) a plan the kernels cannot run exactly: shared memory over budget, too
  * many slots for one pass, the root layouts anywhere but at an unsampled level 0 with every row in slot 0, k_hist2 with
- * more than 2 slots, k_hist_seg at level 0 or with a slot window, a layout other than the shared one with a second plane, or a packed layout (k_hist_seg's included) whose chunk lets a bin
+ * more than 2 slots, k_hist_seg at level 0 or with a slot window, k_hist_root_rows with other than 4 features per lane or
+ * with a slot window, a layout other than the shared one with a second plane, or a packed layout (k_hist_seg's included) whose chunk lets a bin
  * of some feature receive more than 8191 rows (or is not a whole number of the 8-block sub-chunks above 4M rows).  Only scratch that every training iteration rewrites is overwritten. */
 int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* plan, const float* gradients,
                               const float* second, const int32_t* slot_of_row, int32_t n_slots, uint64_t* out_sum,

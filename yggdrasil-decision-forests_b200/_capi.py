@@ -55,9 +55,12 @@ HIST_ROOT_SUM, HIST_PACKED, HIST_SHARED, HIST2, HIST_SEGMENTED = 0, 1, 2, 3, 4  
 
 
 class HistPlan(C.Structure):
-    """One level's k_hist / k_hist2 / k_hist_seg launch (ygg_hist_plan)."""
+    """One level's k_hist / k_hist2 / k_hist_seg / k_hist_root_rows launch (ygg_hist_plan)."""
     _fields_ = [("mode", C.c_int32), ("group", C.c_int32), ("hist2_tiles", C.c_int32), ("chunk_blocks", C.c_int32),
                 ("slot_window", C.c_int32), ("grid", C.c_int32)]
+
+    # the C union {hist2_tiles; root_lanes}: a ROOT_SUM plan's feature lanes (0: k_hist, 32: k_hist_root_rows)
+    root_lanes = property(lambda self: self.hist2_tiles, lambda self, v: setattr(self, "hist2_tiles", v))
 
     def __repr__(self):
         return "HistPlan(%s)" % ", ".join("%s=%d" % (k, getattr(self, k)) for k, _ in self._fields_)

@@ -31,6 +31,7 @@
 #include "ygg_kernels.cuh"
 #include "ygg_wide.cuh"
 #include "ygg_presort.cuh"
+#include "ygg_hist_root.cuh"
 #include "ygg_hist_seg.cuh"
 
 using namespace ygg;
@@ -133,6 +134,7 @@ struct HistLaunch {
   int window, passes;  // window > 0: k_hist<., ., MULTI> over `passes` windows of `window` slots
   int FL, T;           // FL > 0: k_hist2 with FL feature lanes and T sub-tiles per tile
   int SL;              // SL > 0: k_hist_seg with SL feature lanes over S slots (mode kHistPacked, no window)
+  int RL;              // RL > 0: k_hist_root_rows with RL feature lanes of G features each (mode kHistRootSum, level 0)
 };
 
 struct ygg_gbt {
@@ -538,7 +540,7 @@ int chunk_max_count(ygg_gbt* h, int chunk_blocks, uint32_t** d_sub, uint32_t* ou
 }
 
 // Raises the dynamic shared-memory cap of every histogram kernel to its budget, once per device: the seven k_hist
-// instantiations for_hist_kernel returns, the six of k_hist2 and the four of k_hist_seg.  The cap only allows a launch
+// instantiations for_hist_kernel returns, the six of k_hist2, the four of k_hist_seg and k_hist_root_rows.  The cap only allows a launch
 // to request that much
 // (every launch passes its exact size); it is per kernel and shared by every handle of the process (several handles
 // with different feature shards may coexist), hence always the full budget.
@@ -573,6 +575,7 @@ int raise_hist_smem_caps_once(int device) {
   YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<32, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<16, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   YGG_CUDA(cudaFuncSetAttribute(k_hist_seg<8, 1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  YGG_RETURN_IF_ERROR(set_cap(kRootSmemBytes)(k_hist_root_rows));
   done[device] = 1;
   return YGG_OK;
 }
@@ -660,6 +663,7 @@ int configure_launches(ygg_gbt* h) {
     const int n_fgroups = pl.FL > 0 ? (n_groups + pl.FL / 4 - 1) / (pl.FL / 4) : (f_count + G - 1) / G;
     pl.chunk = choose_chunk(n_fgroups, pl.grid, packed ? kSubBlocks : 1, pl.FL > 0 ? min_items2 : min_items);
     pl.SL = 0;
+    pl.RL = 0;
     khist_plan[l] = pl;
     // k_hist_seg (one slot per CTA, node-segmented rows of the row-major copy; ygg_hist_seg.cuh) on the packed levels below
     // the root with at least kSegMinSlots slots, and on levels 1-2 too for wide, large shards (seg_min_slots): below the
@@ -717,6 +721,22 @@ int configure_launches(ygg_gbt* h) {
     }
     dev_free(d_sub);
     if (status != YGG_OK) return status;
+  }
+  // k_hist_root_rows (lanes = features over the row-major copy; ygg_hist_root.cuh) at an unsampled root without a second
+  // plane, on the wide, large shards whose levels 1-2 take k_hist_seg (seg_min_slots), so that the copy is built anyway
+  // (DESIGN.md §5).  Its rows are dense and every item equal: the chunk fills whole waves, with no minimum of items per CTA.
+  if (h->num_levels > 0 && h->hist_plan[0].mode == kHistRootSum && h->hist_plan[0].FL == 0 &&
+      seg_min_slots(f_count, h->ds->n) == 1) {
+    bool seg = false;
+    for (int l = 1; l < h->num_levels; l++) seg |= h->hist_plan[l].SL > 0;
+    if (seg) {
+      HistLaunch& pl = h->hist_plan[0];
+      pl.RL = kRootLanes;
+      pl.G = kRootFpl;
+      pl.S = 1;
+      pl.grid = h->ds->num_sms;
+      pl.chunk = choose_chunk(seg_feature_groups(kRootLanes, kRootFpl, h->hist_f_begin, f_count), pl.grid, 1, 0.0);
+    }
   }
   // k_partition shared accumulators: up to 32 KB (one copy) / 14 KB (lane-private, <= 16 children).
   h->part_smem_children = static_cast<int>((32 * 1024) / (kPartWords * sizeof(uint32_t)));
@@ -1106,6 +1126,20 @@ int launch_hist_seg(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* leve
   return check_launch("k_hist_seg");
 }
 
+// k_hist_root_rows at the root (the counts are copied by accumulate_level).
+int launch_hist_root_rows(ygg_gbt* h, const LevelBuf& lb, const HistLaunch& pl) {
+  ygg_dataset* ds = h->ds;
+  YGG_RETURN_IF_ERROR(ensure_bins_rows(ds));
+  RootRowsParams rp{};
+  rp.rows = ds->d_bins_rows; rp.row_bytes = static_cast<uint32_t>(seg_row_bytes(ds->F));
+  rp.q24 = h->d_q24; rp.act_count = h->d_act_count; rp.n_blocks = h->n_blocks; rp.chunk_blocks = pl.chunk;
+  rp.f_begin = h->hist_f_begin; rp.f_count = h->hist_f_end - h->hist_f_begin;
+  rp.hist_sum = lb.sum; rp.f_chunk = lb.f_chunk; rp.chunk_stride = static_cast<long long>(lb.chunk_u64);
+  k_hist_root_rows<<<pl.grid, kRootThreads, kRootSmemBytes, h->stream>>>(rp);
+  h->launches_total++;
+  return check_launch("k_hist_root_rows");
+}
+
 // Root count histogram: once per (dataset, shard).
 int ensure_root_counts(ygg_gbt* h) {
   if (h->root_cnt_valid) return YGG_OK;
@@ -1139,6 +1173,7 @@ int accumulate_level(ygg_gbt* h, int l, const LevelBuf& lb, const LevelDesc* lev
                                cudaMemcpyDeviceToDevice, h->stream));
   }
   if (pl.SL > 0) return launch_hist_seg(h, l, lb, levels, pl);
+  if (pl.RL > 0) return launch_hist_root_rows(h, lb, pl);
   if (pl.FL > 0) {
     YGG_RETURN_IF_ERROR(ensure_bins4(h->ds));
     Hist2Params hp{};
@@ -3737,6 +3772,7 @@ int ygg_debug_hist_plan(const ygg_gbt* h, int32_t level, ygg_hist_plan* out) {
   } else {
     p.mode = pl.mode == kHistRootSum ? YGG_HIST_ROOT_SUM : pl.mode == kHistPacked ? YGG_HIST_PACKED : YGG_HIST_SHARED;
     p.group = pl.G;
+    p.root_lanes = pl.RL;
   }
   p.chunk_blocks = pl.chunk;
   p.slot_window = pl.window;
@@ -3776,8 +3812,12 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
   } else {
     const ygg_hist_plan& p = *plan;
     if (p.mode < YGG_HIST_ROOT_SUM || p.mode > YGG_HIST_SEGMENTED) return set_error(YGG_ERR_INVALID_ARGUMENT, "unknown mode %d", p.mode);
-    if (p.chunk_blocks < 1 || p.chunk_blocks > kHistMaxChunkBlocks)
-      return set_error(YGG_ERR_INVALID_ARGUMENT, "chunk_blocks=%d outside [1, %d]", p.chunk_blocks, kHistMaxChunkBlocks);
+    const bool root_rows = p.mode == YGG_HIST_ROOT_SUM && p.root_lanes != 0;
+    if (root_rows && p.root_lanes != kRootLanes)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "root_lanes=%d: 0 (k_hist) or %d (k_hist_root_rows)", p.root_lanes, kRootLanes);
+    const int max_chunk = root_rows ? kRootRowsMaxChunkBlocks : kHistMaxChunkBlocks;
+    if (p.chunk_blocks < 1 || p.chunk_blocks > max_chunk)
+      return set_error(YGG_ERR_INVALID_ARGUMENT, "chunk_blocks=%d outside [1, %d]", p.chunk_blocks, max_chunk);
     if (p.grid < 1 || p.grid > 65535) return set_error(YGG_ERR_INVALID_ARGUMENT, "grid=%d outside [1, 65535]", p.grid);
     if (p.slot_window < 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "slot_window=%d", p.slot_window);
     pl.chunk = p.chunk_blocks; pl.grid = p.grid;
@@ -3797,6 +3837,11 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
       if (p.slot_window != 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist_seg has no multi-pass form");
       pl.SL = p.group; pl.S = n_slots; pl.G = 1; pl.passes = 1;
       pl.mode = kHistPacked;
+    } else if (root_rows) {
+      if (p.group != kRootFpl) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist_root_rows: group=%d features per lane (%d)", p.group, kRootFpl);
+      if (p.slot_window != 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "the root layout has no multi-pass form");
+      pl.RL = p.root_lanes; pl.G = p.group; pl.S = n_slots; pl.passes = 1;
+      pl.mode = kHistRootSum;
     } else {
       if (p.group < 1 || p.group > 8) return set_error(YGG_ERR_INVALID_ARGUMENT, "k_hist: group=%d outside [1, 8]", p.group);
       pl.mode = p.mode == YGG_HIST_ROOT_SUM ? kHistRootSum : p.mode == YGG_HIST_PACKED ? kHistPacked : kHistShared;
@@ -3814,7 +3859,7 @@ int ygg_debug_level_histogram(ygg_gbt* h, int32_t level, const ygg_hist_plan* pl
                          pl.G, pl.S, hist_smem_bytes(pl.G, pl.S, hh, pl.mode), budget);
     }
   }
-  if (hh && (pl.FL > 0 || pl.SL > 0 || pl.mode != kHistShared))
+  if (hh && (pl.FL > 0 || pl.SL > 0 || pl.RL > 0 || pl.mode != kHistShared))
     return set_error(YGG_ERR_INVALID_ARGUMENT, "a second histogram plane is accumulated by the shared layout only");
   if (pl.mode == kHistRootSum && (level != 0 || sampling(h) || !all_slot0 || n_slots != 1))
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the root layouts need level 0, no row sampling and every row in slot 0");

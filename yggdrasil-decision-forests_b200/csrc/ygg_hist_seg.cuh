@@ -55,9 +55,10 @@ inline int seg_min_slots(int f_count, long long rows) {
 }
 // Shared memory of a work item of FI = FL x FPL features.
 __host__ __device__ inline size_t seg_smem_bytes(int FI) { return static_cast<size_t>(kMaxBins) * 2 * FI * 4; }
-// Feature groups of a shard: FPL = 2 starts its groups at the even byte at or below the shard's first feature.
+// Feature groups of a shard: FPL = 2 (4) starts its groups at the byte at or below the shard's first feature that is a
+// multiple of 2 (4), so that every lane's FPL-byte load is aligned.
 __host__ __device__ inline int seg_feature_groups(int FL, int FPL, int f_begin, int f_count) {
-  const int off = FPL == 2 ? (f_begin & 1) : 0;
+  const int off = f_begin & (FPL - 1);
   return (f_count + off + FL * FPL - 1) / (FL * FPL);
 }
 // Bytes per row of the row-major copy: the power of two >= F from 32 to 256 (a row is one aligned region of at most
