@@ -206,6 +206,14 @@ int ygg_dataset_set_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t
  * ygg_gbt_create, single GPU, validation / prediction datasets with the same wide columns. */
 int ygg_dataset_set_wide_categorical_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins,
                                             int32_t na_bin);
+/* Discretized wide column (DESIGN.md §25): a numerical feature discretized into num_bins = 257..65535 bins by
+ * GenDiscretizedBoundaries (ygg_dataset_builder_add_numerical16_async makes such columns on the GPU), codes[r] < num_bins
+ * the bin of row r (missing values already folded into na_bin, the bin of the column mean).  It has no bucket values: it is
+ * split by the discretized threshold rule of the byte columns (bucket interpolation), so ygg_node.threshold_bin is a bin
+ * index, threshold_value is NaN and na_value = na_bin >= threshold_bin.  Same rules as ygg_dataset_set_wide_column: before
+ * ygg_gbt_create, single GPU, validation / prediction datasets with the same wide columns. */
+int ygg_dataset_set_wide_discretized_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins,
+                                            int32_t na_bin);
 /* Read-back of a wide column: codes[n_rows], and (may be NULL) its num_bins / na_bin. */
 int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t* codes, int32_t* num_bins, int32_t* na_bin);
 /* Presorted numerical column (DESIGN.md §22): a numerical feature stored as its float values, with no limit on its

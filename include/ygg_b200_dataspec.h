@@ -28,6 +28,11 @@ int ygg_discretize_boundaries(const float* values, int64_t n, int32_t maximum_nu
                               int32_t min_obs_in_bins, float* out_boundaries, int32_t capacity,
                               int32_t* out_num_boundaries, double* out_mean);
 
+/* ygg_discretize_boundaries for maximum_num_bins in [2, 65535]: up to 65535 bins, for uint16 codes. */
+int ygg_discretize_boundaries16(const float* values, int64_t n, int32_t maximum_num_bins,
+                                int32_t min_obs_in_bins, float* out_boundaries, int32_t capacity,
+                                int32_t* out_num_boundaries, double* out_mean);
+
 /* NumericalToDiscretizedNumerical (dataset/data_spec.cc:1006-1018): bin = upper_bound(boundaries, x);
  * missing values are folded into na_bin (see ygg_dataset_create). */
 int ygg_discretize_encode(const float* values, int64_t n, const float* boundaries,
@@ -62,6 +67,12 @@ int ygg_dataset_builder_add_numerical_async(ygg_dataset_builder* b, int32_t feat
 int ygg_dataset_builder_get_numerical(ygg_dataset_builder* b, int32_t feature, float* out_boundaries,
                                       int32_t capacity, int32_t* out_num_boundaries, double* out_mean,
                                       int32_t* out_na_bin, int64_t* out_num_missing);
+/* The same rule for maximum_num_bins in [257, 65535] (DESIGN.md §25): the column becomes a discretized wide column
+ * (ygg_dataset_set_wide_discretized_column) of uint16 codes when the builder is finished, or a byte column when its
+ * boundaries leave at most 256 bins.  Collected with ygg_dataset_builder_get_numerical like the byte columns. */
+int ygg_dataset_builder_add_numerical16_async(ygg_dataset_builder* b, int32_t feature, const float* values,
+                                              int64_t n_stats_rows, int32_t maximum_num_bins,
+                                              int32_t min_obs_in_bins);
 /* A column that is already bucketised on the host (categorical dictionary indices, or bins made by
  * ygg_discretize_encode): n_rows bytes. */
 int ygg_dataset_builder_add_bins(ygg_dataset_builder* b, int32_t feature, const uint8_t* bins, int32_t num_bins,

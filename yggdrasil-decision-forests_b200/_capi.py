@@ -94,6 +94,7 @@ EXPORTS = [
     "ygg_debug_capture_candidates", "ygg_debug_level_candidates",
     "ygg_num_candidate_attributes", "ygg_candidate_key", "ygg_gbt_set_candidate_sampling", "ygg_debug_level_tried",
     "ygg_gbt_set_dart", "ygg_gbt_get_dart_weights", "ygg_gbt_get_dart_dropped",
+    "ygg_dataset_set_wide_discretized_column", "ygg_dataset_builder_add_numerical16_async", "ygg_discretize_boundaries16",
 ]
 
 
@@ -202,6 +203,18 @@ class Dataset:
         most_frequent_value missing values were folded into.  The feature must already be FEATURE_CATEGORICAL."""
         c = np.ascontiguousarray(codes, dtype=np.uint16)
         check(lib().ygg_dataset_set_wide_categorical_column(self.handle, C.c_int32(int(feature)), ptr(c, C.c_uint16),
+                                                            C.c_int64(len(c)), C.c_int32(int(num_bins)), C.c_int32(int(na_bin))))
+        self.num_bins = self.num_bins.copy()
+        self.na_bin = self.na_bin.copy()
+        self.num_bins[feature], self.na_bin[feature] = 1, 0   # the byte column is a one-bucket filler
+        self.wide = dict(getattr(self, "wide", {}))
+        self.wide[int(feature)] = (int(num_bins), int(na_bin))
+
+    def set_wide_discretized_column(self, feature, codes, num_bins, na_bin):
+        """Discretized wide column (257..65535 bins of GenDiscretizedBoundaries): codes[r] = the uint16 bin of row r,
+        na_bin = the bin of the column mean missing values were folded into.  Split by the discretized threshold rule."""
+        c = np.ascontiguousarray(codes, dtype=np.uint16)
+        check(lib().ygg_dataset_set_wide_discretized_column(self.handle, C.c_int32(int(feature)), ptr(c, C.c_uint16),
                                                             C.c_int64(len(c)), C.c_int32(int(num_bins)), C.c_int32(int(na_bin))))
         self.num_bins = self.num_bins.copy()
         self.na_bin = self.na_bin.copy()
@@ -323,14 +336,33 @@ class DatasetBuilder:
             C.c_int32(maximum_num_bins), C.c_int32(min_obs_in_bins)))
         self.h2d_bytes += v.nbytes
 
+    def add_numerical16_async(self, feature, values, maximum_num_bins, min_obs_in_bins=3, n_stats_rows=0):
+        """add_numerical_async for 257..65535 bins: a column that ends with more than 256 bins becomes a discretized
+        wide column (uint16 codes) when the builder is finished, one with fewer a byte column."""
+        v = np.ascontiguousarray(values, dtype=np.float32)
+        assert v.shape == (self.n_rows,)
+        self._pending = getattr(self, "_pending", {})
+        check(lib().ygg_dataset_builder_add_numerical16_async(
+            self.handle, C.c_int32(feature), ptr(v, C.c_float), C.c_int64(n_stats_rows),
+            C.c_int32(maximum_num_bins), C.c_int32(min_obs_in_bins)))
+        self._pending[feature] = v
+        self._wide16 = getattr(self, "_wide16", set()) | {int(feature)}
+        self.h2d_bytes += v.nbytes
+
     def get_numerical(self, feature):
-        bounds = np.empty(256, np.float32)
+        wide16 = int(feature) in getattr(self, "_wide16", ())
+        capacity = 65535 if wide16 else 256
+        bounds = np.empty(capacity, np.float32)
         nb, mean, na, miss = C.c_int32(), C.c_double(), C.c_int32(), C.c_int64()
         check(lib().ygg_dataset_builder_get_numerical(self.handle, C.c_int32(feature), ptr(bounds, C.c_float),
-                                                      C.c_int32(256), C.byref(nb), C.byref(mean), C.byref(na),
+                                                      C.c_int32(capacity), C.byref(nb), C.byref(mean), C.byref(na),
                                                       C.byref(miss)))
         getattr(self, "_pending", {}).pop(feature, None)
         self.num_bins[feature], self.na_bin[feature] = nb.value + 1, na.value
+        if wide16 and nb.value + 1 > 256:   # a discretized wide column at finish: its byte column is a one-bucket filler
+            self.num_bins[feature], self.na_bin[feature] = 1, 0
+            self.wide = dict(getattr(self, "wide", {}))
+            self.wide[int(feature)] = (nb.value + 1, na.value)
         return bounds[:nb.value].copy(), mean.value, na.value, miss.value
 
     def add_bins(self, feature, bins, num_bins, na_bin, feature_type=0):
@@ -339,6 +371,9 @@ class DatasetBuilder:
         check(lib().ygg_dataset_builder_add_bins(self.handle, C.c_int32(feature), ptr(b, C.c_uint8),
                                                  C.c_int32(num_bins), C.c_int32(na_bin), C.c_int32(feature_type)))
         self.num_bins[feature], self.na_bin[feature], self.feature_types[feature] = num_bins, na_bin, feature_type
+        if int(feature) in getattr(self, "_wide16", ()):
+            self._wide16.discard(int(feature))
+            getattr(self, "wide", {}).pop(int(feature), None)
         self.h2d_bytes += b.nbytes
 
     def finish(self):
@@ -353,6 +388,8 @@ class DatasetBuilder:
         ds.n_features, ds.n_rows = self.n_features, self.n_rows
         ds.num_bins, ds.na_bin, ds.feature_types = self.num_bins, self.na_bin, self.feature_types
         ds.h2d_bytes = self.h2d_bytes
+        if getattr(self, "wide", None):
+            ds.wide = dict(self.wide)
         return ds
 
     def close(self):
@@ -856,6 +893,19 @@ def discretize_boundaries(values, maximum_num_bins=255, min_obs_in_bins=3):
                                           C.c_int32(maximum_num_bins), C.c_int32(min_obs_in_bins),
                                           ptr(out, C.c_float), C.c_int32(len(out)), C.byref(n),
                                           C.byref(mean)))
+    return out[:n.value].copy(), mean.value
+
+
+def discretize_boundaries16(values, maximum_num_bins, min_obs_in_bins=3):
+    """discretize_boundaries for maximum_num_bins in [2, 65535] (up to 65535 bins, for uint16 codes)."""
+    v = np.ascontiguousarray(values, dtype=np.float32)
+    out = np.zeros(maximum_num_bins + 4, dtype=np.float32)
+    n = C.c_int32()
+    mean = C.c_double()
+    check(lib().ygg_discretize_boundaries16(ptr(v, C.c_float), C.c_int64(len(v)),
+                                            C.c_int32(maximum_num_bins), C.c_int32(min_obs_in_bins),
+                                            ptr(out, C.c_float), C.c_int32(len(out)), C.byref(n),
+                                            C.byref(mean)))
     return out[:n.value].copy(), mean.value
 
 

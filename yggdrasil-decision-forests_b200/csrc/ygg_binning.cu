@@ -1,5 +1,6 @@
 // ygg_binning.cu — on-GPU dataspec step in front of the split finder (SURVEY.md §8f N1): float32 columns
-// -> discretization boundaries -> uint8 bins written straight into the device-resident dataset.
+// -> discretization boundaries -> uint8 bins written straight into the device-resident dataset (or, above 256
+// bins, uint16 codes that become a discretized wide column, DESIGN.md §25).
 //
 // Same rule as the host path (ygg_dataspec.cc), i.e. the reference's
 //   GenDiscretizedBoundaries                 dataset/data_spec.cc:854-986
@@ -20,6 +21,10 @@
 //                   <= 255 searches instead of 10^7 sequential steps — identical cuts, proven against
 //                   the host rule bit for bit in tests/test_gpu_binning.py;
 //   k_bin_encode    bin = upper_bound(boundaries, x), NaN -> the bin of the mean.
+// Up to 65535 bins (ygg_dataset_builder_add_numerical16_async, DESIGN.md §25) the sort, distinct-value and mean kernels
+// are the same; the large candidates are listed in order by a compaction (k_bin_large_count / _write), the cuts are walked
+// by k_bin_boundaries16 with its lists in global memory, k_bin_specials16 inserts the special values' bins, and
+// k_bin_encode16 writes uint16 codes through a two-level search.
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -40,6 +45,11 @@ constexpr int kSortTile = kSortThreads * kSortRounds;           // 8192 keys per
 constexpr int kMaxBoundaries = 255;
 constexpr int kMaxLarge = 1024;                                 // >= 2 * maximum_num_bins (see k_bin_find_large)
 constexpr uint32_t kNanKey = 0xFFFFFFFFu;
+constexpr int kMaxBoundaries16 = 65534;                         // uint16 codes 0..65534
+constexpr int kBoundaries16Cap = kMaxBoundaries16 + 8;          // room for the special values' bins before the check
+constexpr int kMaxLarge16 = 2 * 65536;                          // >= 2 * maximum_num_bins
+constexpr int kCoarseStep = 64;                                 // k_bin_encode16: boundaries per coarse entry
+constexpr int kCoarse = 1024;                                   // coarse entries (kCoarse * kCoarseStep > kMaxBoundaries16)
 
 struct BinState {
   unsigned long long n_valid;   // non-missing values
@@ -551,6 +561,244 @@ __global__ void __launch_bounds__(256) k_bin_encode(const float* __restrict__ va
   }
 }
 
+// ---- up to 65535 bins ---------------------------------------------------------------------------
+// The large candidates (count >= st->large) in increasing order: per tile of kSortTile candidates a count, scanned, then
+// written at their offsets.  st->n_large = their number; more than kMaxLarge16 sets st->error.
+__device__ __forceinline__ bool is_large(const uint32_t* pos, int64_t u, uint32_t nc, long long large) {
+  return u < static_cast<int64_t>(nc) && static_cast<long long>(pos[u + 1] - pos[u]) >= large;
+}
+
+__global__ void __launch_bounds__(kSortThreads) k_bin_large_count(const uint32_t* __restrict__ pos, const BinState* st,
+                                                                  uint32_t* __restrict__ tile_count) {
+  __shared__ unsigned int s_total;
+  if (threadIdx.x == 0) s_total = 0;
+  __syncthreads();
+  unsigned int c = 0;
+  if (st->mode == 1) {
+    const uint32_t nc = st->nc;
+    const long long large = st->large;
+    const int64_t base = static_cast<int64_t>(blockIdx.x) * kSortTile + static_cast<int64_t>(threadIdx.x) * kSortRounds;
+#pragma unroll
+    for (int r = 0; r < kSortRounds; r++) c += is_large(pos, base + r, nc, large) ? 1u : 0u;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(&s_total, c);
+  __syncthreads();
+  if (threadIdx.x == 0) tile_count[blockIdx.x] = s_total;
+}
+
+__global__ void __launch_bounds__(kSortThreads) k_bin_large_write(const uint32_t* __restrict__ pos, BinState* st,
+                                                                  const uint32_t* __restrict__ tile_offset /*scanned*/,
+                                                                  const uint32_t* __restrict__ total,
+                                                                  uint32_t* __restrict__ large_idx) {
+  __shared__ uint32_t s_warp[kSortWarps];
+  if (st->mode != 1) return;
+  const uint32_t nc = st->nc;
+  const long long large = st->large;
+  const int64_t base = static_cast<int64_t>(blockIdx.x) * kSortTile + static_cast<int64_t>(threadIdx.x) * kSortRounds;
+  uint32_t flags = 0, c = 0;
+#pragma unroll
+  for (int r = 0; r < kSortRounds; r++)
+    if (is_large(pos, base + r, nc, large)) { flags |= 1u << r; c++; }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t inc = c;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t x = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += x;
+  }
+  if (lane == 31) s_warp[w] = inc;
+  __syncthreads();
+  uint32_t off = tile_offset[blockIdx.x] + (inc - c);
+  for (int i = 0; i < w; i++) off += s_warp[i];
+#pragma unroll
+  for (int r = 0; r < kSortRounds; r++)
+    if (flags & (1u << r)) {
+      if (off < static_cast<uint32_t>(kMaxLarge16)) large_idx[off] = static_cast<uint32_t>(base + r);
+      off++;
+    }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    st->n_large = *total;
+    if (*total > static_cast<uint32_t>(kMaxLarge16)) st->error = 1;
+  }
+}
+
+// k_bin_boundaries' walk with its lists in global memory: `large_idx` sorted (k_bin_large_write), the cuts in `cut`
+// [kMaxBoundaries16], their midpoints in `mids` and their number in st->num_boundaries (before the special values).
+__global__ void __launch_bounds__(32) k_bin_boundaries16(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ pos,
+                                                         const uint32_t* __restrict__ large_idx, int min_obs, BinState* st,
+                                                         uint32_t* __restrict__ cut, float* __restrict__ mids) {
+  const int lane = threadIdx.x;
+  const uint32_t nc = st->nc;
+  const unsigned long long total = st->n_valid;
+  int nb = 0;
+  bool overflow = st->error != 0;
+  auto value = [&](uint32_t u) { return key_to_float(keys[pos[u]]); };
+  if (st->mode == 0) {
+    if (lane == 0) {
+      long long running = 0;
+      for (uint32_t i = 0; i + 1 < nc; i++) {  // nc <= max_bins <= 65533 here
+        running += pos[i + 1] - pos[i];
+        if (running >= min_obs) {
+          if (nb < kMaxBoundaries16) cut[nb++] = i; else overflow = true;
+          running = 0;
+        }
+      }
+    }
+    nb = __shfl_sync(0xffffffffu, nb, 0);
+  } else if (!overflow) {
+    const uint32_t nL = st->n_large;
+    const int max_boundaries = st->max_bins - 1;
+    long long lsum_all = 0;
+    for (uint32_t i = lane; i < nL; i += 32) lsum_all += pos[large_idx[i] + 1] - pos[large_idx[i]];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) lsum_all += __shfl_xor_sync(0xffffffffu, lsum_all, o);
+    const long long total_nonlarge = static_cast<long long>(total) - lsum_all;
+    long long remaining_bins = static_cast<long long>(st->max_bins_eff) - nL;
+    if (remaining_bins < 1) remaining_bins = 1;
+    long long cur_large = total_nonlarge / remaining_bins;
+    uint32_t s = 0, li = 0;
+    long long lsum = 0;  // counts of the large candidates with index < s
+    int made = 0;
+    while (static_cast<unsigned long long>(s) + 2 <= nc) {
+      const uint32_t next_large = li < nL ? large_idx[li] : 0xFFFFFFFFu;   // first large index >= s
+      const unsigned long long ps = pos[s];
+      // (a) running >= cur_large: first i >= s with pos[i+1] - pos[s] >= cur_large
+      uint32_t i_a;
+      if (cur_large <= 0) {
+        i_a = s;
+      } else {
+        const uint32_t j = warp_lower_bound(pos, s + 1, nc + 1, ps + static_cast<unsigned long long>(cur_large));
+        i_a = j <= nc ? j - 1 : 0xFFFFFFFFu;
+      }
+      // (b) the next large candidate cuts at its own index; (c) the candidate before it cuts early
+      uint32_t i_star = min(i_a, next_large);
+      if (next_large != 0xFFFFFFFFu && next_large >= s + 1) {
+        const long long half = cur_large / 2 > 1 ? cur_large / 2 : 1;
+        if (static_cast<long long>(pos[next_large] - ps) >= half) i_star = min(i_star, next_large - 1);
+      }
+      if (static_cast<unsigned long long>(i_star) + 2 > nc) break;     // the loop stops at nc - 2
+      if (lane == 0) {
+        if (nb < kMaxBoundaries16) cut[nb] = i_star; else overflow = true;
+      }
+      nb++;
+      if (++made >= max_boundaries) break;   // checked after the push, as the reference does
+      const bool large_cut = i_star == next_large;
+      if (large_cut) { lsum += pos[next_large + 1] - pos[next_large]; li++; }
+      const long long remaining = total_nonlarge - (static_cast<long long>(pos[i_star + 1]) - lsum);
+      if (!large_cut) {
+        remaining_bins = remaining_bins - 1 < 1 ? 1 : remaining_bins - 1;
+        cur_large = remaining / remaining_bins;
+      }
+      s = i_star + 1;
+    }
+    if (nb > kMaxBoundaries16) { nb = kMaxBoundaries16; overflow = true; }
+  }
+  __syncwarp();
+  // boundary = midpoint of the candidates around each cut (float arithmetic, as the reference); non-decreasing
+  for (int k = lane; k < nb; k += 32) mids[k] = (value(cut[k]) + value(cut[k] + 1)) / 2;
+  if (lane == 0) {
+    st->num_boundaries = nb;
+    if (overflow) st->error = 1;
+  }
+}
+
+// add_special_bucket on a SORTED boundary list `in` [n], written sorted to `out` (all threads of the CTA): the entries
+// inside [v - ulp, v + ulp] go, v - ulp comes in when an entry stays below it, v + ulp when one stays above it, both
+// when none stays.  The host rule appends and sorts at the end; the sorted list is the same.
+__device__ int special_pass16(const float* __restrict__ in, int n, float v, float* __restrict__ out, int* s_i) {
+  const float lo = nextafterf(v, v - 1.f), hi = nextafterf(v, v + 1.f);
+  if (threadIdx.x == 0) {
+    int a = 0, b = n;   // first entry >= lo
+    while (a < b) { const int m = (a + b) >> 1; if (in[m] < lo) a = m + 1; else b = m; }
+    s_i[0] = a;
+    b = n;              // first entry > hi
+    while (a < b) { const int m = (a + b) >> 1; if (in[m] <= hi) a = m + 1; else b = m; }
+    s_i[1] = a;
+  }
+  __syncthreads();
+  const int i0 = s_i[0], i1 = s_i[1];
+  __syncthreads();
+  const bool none_left = i0 == 0 && i1 == n;
+  const int extra = none_left ? 2 : (i0 > 0 ? 1 : 0) + (i1 < n ? 1 : 0);
+  const int n_out = i0 + extra + (n - i1);
+  for (int k = threadIdx.x; k < n_out; k += blockDim.x) {
+    float x;
+    if (k < i0) x = in[k];
+    else if (k - i0 < extra) x = (k == i0 && (none_left || i0 > 0)) ? lo : hi;
+    else x = in[i1 + (k - i0 - extra)];
+    out[k] = x;
+  }
+  __syncthreads();
+  return n_out;
+}
+
+// One CTA: the special values {0, mean} (as k_bin_boundaries), the count check and na_bin = upper_bound(boundaries, mean).
+__global__ void __launch_bounds__(1024) k_bin_specials16(BinState* st, const float* __restrict__ mids, float* __restrict__ tmp,
+                                                         float* __restrict__ out) {
+  __shared__ int s_i[2];
+  const int nb0 = st->num_boundaries;
+  const float m = static_cast<float>(st->mean);
+  const int nb1 = special_pass16(mids, nb0, 0.f, tmp, s_i);
+  const int nb = special_pass16(tmp, nb1, m, out, s_i);
+  if (threadIdx.x == 0) {
+    int a = 0, b = nb;   // upper_bound(boundaries, (float)mean)
+    while (a < b) { const int k = (a + b) >> 1; if (out[k] <= m) a = k + 1; else b = k; }
+    st->num_boundaries = nb;
+    st->na_bin = a;
+    if (nb > kMaxBoundaries16) st->error = 1;
+  }
+}
+
+// bin = upper_bound(boundaries, x) over up to 65534 boundaries, NaN -> the bin of the mean: the coarse table (every
+// kCoarseStep-th boundary) in shared memory picks a run of kCoarseStep - 1 boundaries, searched in global memory (L2).
+__global__ void __launch_bounds__(256) k_bin_encode16(const float* __restrict__ values, int64_t n, const BinState* st,
+                                                      const float* __restrict__ boundaries, uint16_t* __restrict__ out) {
+  __shared__ float s_c[kCoarse];
+  const int nb = min(st->num_boundaries, kMaxBoundaries16);
+  const int na = st->na_bin;
+  const float inf = __int_as_float(0x7f800000);
+  for (int k = threadIdx.x; k < kCoarse; k += blockDim.x) {
+    const int i = (k + 1) * kCoarseStep - 1;
+    s_c[k] = i < nb ? boundaries[i] : inf;   // +inf padding
+  }
+  __syncthreads();
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n;
+       r += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const float x = values[r];
+    int bin = na;
+    if (x == x) {
+      int c = 0;   // coarse entries <= x
+#pragma unroll
+      for (int step = kCoarse / 2; step > 0; step >>= 1)
+        if (s_c[c + step - 1] <= x) c += step;
+      const int base = c * kCoarseStep;
+      if (base >= nb) {
+        bin = nb;
+      } else {
+        // boundaries [base, base + kCoarseStep - 1) hold the answer; the entry after them is the coarse one, > x
+        int p = 0;
+#pragma unroll
+        for (int step = kCoarseStep / 2; step > 0; step >>= 1) {
+          const int i = p + step - 1;
+          const float b = (i < kCoarseStep - 1 && base + i < nb) ? __ldg(boundaries + base + i) : inf;
+          if (b <= x) p += step;
+        }
+        bin = min(base + p, nb);   // x = +inf passes the padding too
+      }
+    }
+    out[r] = static_cast<uint16_t>(bin);
+  }
+}
+
+// A column binned by the 16-bit path that ended with at most 256 bins: its codes as a byte column.
+__global__ void __launch_bounds__(256) k_bin_narrow16(const uint16_t* __restrict__ in, int64_t n, uint8_t* __restrict__ out) {
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n;
+       r += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    out[r] = static_cast<uint8_t>(in[r]);
+}
+
 #define YGG_BIN_CUDA(expr)                                                                   \
   do {                                                                                       \
     cudaError_t _e = (expr);                                                                 \
@@ -576,6 +824,8 @@ struct ColumnResult {
   int64_t n_stats = 0;
   BinState st{};
   float bounds[256];
+  bool wide16 = false;           // binned by the 16-bit path: its boundaries are in bounds16
+  std::vector<float> bounds16;
 };
 
 struct BinLane {
@@ -592,12 +842,20 @@ struct BinLane {
   float* d_boundaries = nullptr;
   BinState* d_state = nullptr;
   HostResult* h_result = nullptr;
+  // the 16-bit path's lists (allocated on its first column)
+  uint32_t* d_large16 = nullptr;    // [kMaxLarge16]
+  uint32_t* d_cut = nullptr;        // [kBoundaries16Cap]
+  float* d_mids = nullptr;          // [kBoundaries16Cap] each
+  float* d_tmp16 = nullptr;
+  float* d_bounds16 = nullptr;
+  float* h_bounds16 = nullptr;      // pinned
 };
 
 struct ygg_dataset_builder {
   ygg_dataset* ds = nullptr;
   std::vector<char> filled;
   std::vector<ColumnResult> results;
+  std::vector<uint16_t*> codes16;   // [F] device codes of the 16-bit columns with more than 256 bins (attached at finish)
   int64_t n_tiles = 0;
   int next_lane = 0;
   BinLane lane[kRing];
@@ -613,9 +871,12 @@ void free_builder(ygg_dataset_builder* b) {
     cudaFree(l.d_values); cudaFree(l.d_keys[0]); cudaFree(l.d_keys[1]); cudaFree(l.d_pos); cudaFree(l.d_table);
     cudaFree(l.d_chunk); cudaFree(l.d_total); cudaFree(l.d_large); cudaFree(l.d_partial); cudaFree(l.d_boundaries);
     cudaFree(l.d_state);
+    cudaFree(l.d_large16); cudaFree(l.d_cut); cudaFree(l.d_mids); cudaFree(l.d_tmp16); cudaFree(l.d_bounds16);
+    if (l.h_bounds16) cudaFreeHost(l.h_bounds16);
     if (l.h_result) cudaFreeHost(l.h_result);
     if (l.stream) cudaStreamDestroy(l.stream);
   }
+  for (uint16_t* c : b->codes16) cudaFree(c);
   if (b->ds != nullptr) ygg_dataset_destroy(b->ds);
   delete b;
 }
@@ -639,12 +900,58 @@ int ensure_lane(ygg_dataset_builder* b, BinLane* l) {
   return YGG_OK;
 }
 
+int ensure_lane16(BinLane* l) {
+  if (l->d_large16 != nullptr) return YGG_OK;
+  YGG_BIN_CUDA(cudaMalloc(&l->d_large16, sizeof(uint32_t) * kMaxLarge16));
+  YGG_BIN_CUDA(cudaMalloc(&l->d_cut, sizeof(uint32_t) * kBoundaries16Cap));
+  YGG_BIN_CUDA(cudaMalloc(&l->d_mids, sizeof(float) * kBoundaries16Cap));
+  YGG_BIN_CUDA(cudaMalloc(&l->d_tmp16, sizeof(float) * kBoundaries16Cap));
+  YGG_BIN_CUDA(cudaMalloc(&l->d_bounds16, sizeof(float) * kBoundaries16Cap));
+  YGG_BIN_CUDA(cudaMallocHost(&l->h_bounds16, sizeof(float) * kBoundaries16Cap));
+  return YGG_OK;
+}
+
+// Frees the 16-bit codes of a feature that is binned again or replaced.
+void drop_codes16(ygg_dataset_builder* b, int f) {
+  cudaFree(b->codes16[f]);
+  b->codes16[f] = nullptr;
+}
+
 int launch_scan(BinLane* l, uint32_t* data, int64_t count, uint32_t* total_out) {
   const int64_t n_chunks = (count + kScanChunk - 1) / kScanChunk;
   if (n_chunks > kScanChunk) return ygg_set_error_msg(YGG_ERR_UNIMPLEMENTED, "too many rows for the GPU binning path");
   k_scan_local<<<static_cast<int>(n_chunks), 1024, 0, l->stream>>>(data, count, l->d_chunk);
   k_scan_tops<<<1, 1024, 0, l->stream>>>(l->d_chunk, static_cast<int>(n_chunks), total_out);
   k_scan_add<<<static_cast<int>(n_chunks), 1024, 0, l->stream>>>(data, count, l->d_chunk);
+  return YGG_OK;
+}
+
+// retire_lane for a column of the 16-bit path (its stream is idle): a column with at most 256 bins becomes a byte
+// column, a wider one keeps its codes for ygg_dataset_builder_finish.
+int retire_column16(ygg_dataset_builder* b, BinLane* l, int f, ColumnResult* r) {
+  ygg_dataset* ds = b->ds;
+  if (r->st.error != 0 || r->st.num_boundaries > kMaxBoundaries16) {
+    r->status = -1;
+    drop_codes16(b, f);
+    char m[160];
+    std::snprintf(m, sizeof(m), "feature %d needs more than 65535 bins (or has too many heavy values)", f);
+    return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, m);
+  }
+  r->bounds16.assign(l->h_bounds16, l->h_bounds16 + r->st.num_boundaries);
+  const int num_bins = r->st.num_boundaries + 1;
+  ds->feature_type[f] = YGG_FEATURE_DISCRETIZED_NUMERICAL;
+  if (num_bins <= 256) {
+    k_bin_narrow16<<<ds->num_sms * 8, 256, 0, l->stream>>>(b->codes16[f], ds->n, ds->d_bins + static_cast<size_t>(f) * ds->n_pad);
+    YGG_BIN_CUDA(cudaGetLastError());
+    YGG_BIN_CUDA(cudaStreamSynchronize(l->stream));
+    drop_codes16(b, f);
+    ds->num_bins[f] = num_bins;
+    ds->na_bin[f] = r->st.na_bin;
+  } else {   // the byte column becomes the wide column's filler at finish
+    ds->num_bins[f] = 1;
+    ds->na_bin[f] = 0;
+  }
+  b->filled[f] = 1;
   return YGG_OK;
 }
 
@@ -659,6 +966,7 @@ int retire_lane(ygg_dataset_builder* b, BinLane* l) {
   std::memcpy(r.bounds, l->h_result->bounds, sizeof(r.bounds));
   r.status = 0;
   r.lane = -1;
+  if (r.wide16) return retire_column16(b, l, f, &r);
   if (r.st.error != 0 || r.st.num_boundaries > kMaxBoundaries) {
     r.status = -1;
     char m[160];
@@ -673,30 +981,11 @@ int retire_lane(ygg_dataset_builder* b, BinLane* l) {
   return YGG_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-int ygg_dataset_builder_create(ygg_dataset_builder** out, int64_t n_rows, int32_t n_features, int32_t device) {
-  if (out == nullptr) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "null argument");
-  ygg_dataset* ds = nullptr;
-  if (int st = ygg_internal_dataset_alloc(&ds, n_rows, n_features, device)) return st;
-  auto* b = new ygg_dataset_builder();
-  b->ds = ds;
-  b->filled.assign(n_features, 0);
-  b->results.resize(n_features);
-  b->n_tiles = (n_rows + kSortTile - 1) / kSortTile;
-  *out = b;
-  return YGG_OK;
-}
-
-int ygg_dataset_builder_add_numerical_async(ygg_dataset_builder* b, int32_t feature, const float* values,
-                                            int64_t n_stats_rows, int32_t maximum_num_bins, int32_t min_obs_in_bins) {
-  if (!b || !b->ds || !values) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "null argument");
+// The two add_numerical entries once their bin budget is checked: uploads the column and enqueues its kernels on the
+// next lane.  `wide16`: the 16-bit path (up to 65535 bins, uint16 codes kept for finish), else the byte path.
+int enqueue_column(ygg_dataset_builder* b, int32_t feature, const float* values, int64_t n_stats_rows,
+                   int32_t maximum_num_bins, int32_t min_obs_in_bins, bool wide16) {
   ygg_dataset* ds = b->ds;
-  if (feature < 0 || feature >= ds->F) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "feature index out of range");
-  if (maximum_num_bins < 4 || maximum_num_bins > 256)
-    return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "maximum_num_bins must be in [4, 256] on the GPU binning path");
   if (min_obs_in_bins < 1) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "min_obs_in_bins < 1");
   if (b->results[feature].status == 1) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "the feature is already in flight");
   const int64_t n = ds->n;
@@ -709,7 +998,11 @@ int ygg_dataset_builder_add_numerical_async(ygg_dataset_builder* b, int32_t feat
   const int lane_id = b->next_lane;
   b->next_lane = (b->next_lane + 1) % kRing;
   if (int st = ensure_lane(b, l)) return st;
+  if (wide16)
+    if (int st = ensure_lane16(l)) return st;
   if (int st = retire_lane(b, l)) return st;
+  drop_codes16(b, feature);
+  if (wide16) YGG_BIN_CUDA(cudaMalloc(&b->codes16[feature], sizeof(uint16_t) * (n > 0 ? n : 1)));
   cudaStream_t s = l->stream;
   const int n_tiles = static_cast<int>(b->n_tiles);
   YGG_BIN_CUDA(cudaMemcpyAsync(l->d_values, values, sizeof(float) * n, cudaMemcpyHostToDevice, s));
@@ -728,10 +1021,20 @@ int ygg_dataset_builder_add_numerical_async(ygg_dataset_builder* b, int32_t feat
   if (int st = launch_scan(l, l->d_table, n_tiles, l->d_total)) return st;
   k_heads_write<<<n_tiles, kSortThreads, 0, s>>>(sorted, l->d_state, l->d_table, l->d_total, l->d_pos);
   k_bin_prep<<<1, 32, 0, s>>>(sorted, l->d_partial, n_tiles, maximum_num_bins, min_obs_in_bins, l->d_state);
-  k_bin_find_large<<<ds->num_sms * 4, 256, 0, s>>>(l->d_pos, l->d_state, l->d_large);
-  k_bin_boundaries<<<1, 32, 0, s>>>(sorted, l->d_pos, l->d_large, min_obs_in_bins, l->d_state, l->d_boundaries);
-  k_bin_encode<<<ds->num_sms * 8, 256, 0, s>>>(l->d_values, n, l->d_state, l->d_boundaries,
-                                                ds->d_bins + static_cast<size_t>(feature) * ds->n_pad);
+  if (wide16) {
+    k_bin_large_count<<<n_tiles, kSortThreads, 0, s>>>(l->d_pos, l->d_state, l->d_table);
+    if (int st = launch_scan(l, l->d_table, n_tiles, l->d_total)) return st;
+    k_bin_large_write<<<n_tiles, kSortThreads, 0, s>>>(l->d_pos, l->d_state, l->d_table, l->d_total, l->d_large16);
+    k_bin_boundaries16<<<1, 32, 0, s>>>(sorted, l->d_pos, l->d_large16, min_obs_in_bins, l->d_state, l->d_cut, l->d_mids);
+    k_bin_specials16<<<1, 1024, 0, s>>>(l->d_state, l->d_mids, l->d_tmp16, l->d_bounds16);
+    k_bin_encode16<<<ds->num_sms * 8, 256, 0, s>>>(l->d_values, n, l->d_state, l->d_bounds16, b->codes16[feature]);
+    YGG_BIN_CUDA(cudaMemcpyAsync(l->h_bounds16, l->d_bounds16, sizeof(float) * kBoundaries16Cap, cudaMemcpyDeviceToHost, s));
+  } else {
+    k_bin_find_large<<<ds->num_sms * 4, 256, 0, s>>>(l->d_pos, l->d_state, l->d_large);
+    k_bin_boundaries<<<1, 32, 0, s>>>(sorted, l->d_pos, l->d_large, min_obs_in_bins, l->d_state, l->d_boundaries);
+    k_bin_encode<<<ds->num_sms * 8, 256, 0, s>>>(l->d_values, n, l->d_state, l->d_boundaries,
+                                                  ds->d_bins + static_cast<size_t>(feature) * ds->n_pad);
+  }
   YGG_BIN_CUDA(cudaGetLastError());
   YGG_BIN_CUDA(cudaMemcpyAsync(&l->h_result->st, l->d_state, sizeof(BinState), cudaMemcpyDeviceToHost, s));
   YGG_BIN_CUDA(cudaMemcpyAsync(l->h_result->bounds, l->d_boundaries, sizeof(float) * 256, cudaMemcpyDeviceToHost, s));
@@ -740,8 +1043,47 @@ int ygg_dataset_builder_add_numerical_async(ygg_dataset_builder* b, int32_t feat
   r.status = 1;
   r.lane = lane_id;
   r.n_stats = n_stats_rows;
+  r.wide16 = wide16;
   b->filled[feature] = 0;
   return YGG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ygg_dataset_builder_create(ygg_dataset_builder** out, int64_t n_rows, int32_t n_features, int32_t device) {
+  if (out == nullptr) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  ygg_dataset* ds = nullptr;
+  if (int st = ygg_internal_dataset_alloc(&ds, n_rows, n_features, device)) return st;
+  auto* b = new ygg_dataset_builder();
+  b->ds = ds;
+  b->filled.assign(n_features, 0);
+  b->results.resize(n_features);
+  b->codes16.assign(n_features, nullptr);
+  b->n_tiles = (n_rows + kSortTile - 1) / kSortTile;
+  *out = b;
+  return YGG_OK;
+}
+
+int ygg_dataset_builder_add_numerical_async(ygg_dataset_builder* b, int32_t feature, const float* values,
+                                            int64_t n_stats_rows, int32_t maximum_num_bins, int32_t min_obs_in_bins) {
+  if (!b || !b->ds || !values) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  ygg_dataset* ds = b->ds;
+  if (feature < 0 || feature >= ds->F) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "feature index out of range");
+  if (maximum_num_bins < 4 || maximum_num_bins > 256)
+    return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "maximum_num_bins must be in [4, 256] on the GPU binning path");
+  return enqueue_column(b, feature, values, n_stats_rows, maximum_num_bins, min_obs_in_bins, false);
+}
+
+int ygg_dataset_builder_add_numerical16_async(ygg_dataset_builder* b, int32_t feature, const float* values,
+                                              int64_t n_stats_rows, int32_t maximum_num_bins, int32_t min_obs_in_bins) {
+  if (!b || !b->ds || !values) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "null argument");
+  ygg_dataset* ds = b->ds;
+  if (feature < 0 || feature >= ds->F) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "feature index out of range");
+  if (maximum_num_bins < 257 || maximum_num_bins > 65535)
+    return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "maximum_num_bins must be in [257, 65535] on the 16-bit GPU binning path");
+  return enqueue_column(b, feature, values, n_stats_rows, maximum_num_bins, min_obs_in_bins, true);
 }
 
 int ygg_dataset_builder_get_numerical(ygg_dataset_builder* b, int32_t feature, float* out_boundaries, int32_t capacity,
@@ -758,7 +1100,7 @@ int ygg_dataset_builder_get_numerical(ygg_dataset_builder* b, int32_t feature, f
   if (out_num_boundaries) *out_num_boundaries = r.st.num_boundaries;
   if (out_boundaries) {
     if (capacity < r.st.num_boundaries) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "boundary buffer too small");
-    std::memcpy(out_boundaries, r.bounds, sizeof(float) * r.st.num_boundaries);
+    std::memcpy(out_boundaries, r.wide16 ? r.bounds16.data() : r.bounds, sizeof(float) * r.st.num_boundaries);
   }
   if (out_mean) *out_mean = r.st.mean;
   if (out_na_bin) *out_na_bin = r.st.na_bin;
@@ -788,6 +1130,7 @@ int ygg_dataset_builder_add_bins(ygg_dataset_builder* b, int32_t feature, const 
   if (b->results[feature].status == 1) return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, "the feature is in flight");
   YGG_BIN_CUDA(cudaSetDevice(ds->device));
   YGG_BIN_CUDA(cudaMemcpy(ds->d_bins + static_cast<size_t>(feature) * ds->n_pad, bins, ds->n, cudaMemcpyHostToDevice));
+  drop_codes16(b, feature);
   ds->num_bins[feature] = num_bins;
   ds->na_bin[feature] = na_bin;
   ds->feature_type[feature] = feature_type;
@@ -808,6 +1151,16 @@ int ygg_dataset_builder_finish(ygg_dataset_builder* b, ygg_dataset** out) {
       return ygg_set_error_msg(YGG_ERR_INVALID_ARGUMENT, m);
     }
   if (int st = ygg_internal_dataset_finalize(b->ds)) return st;
+  int n16 = 0;
+  for (const uint16_t* c : b->codes16) n16 += c != nullptr ? 1 : 0;
+  if (n16 > 0)   // one allocation for all of them, then each attach copies one plane
+    if (int st = ygg_internal_reserve_wide(b->ds, b->ds->n_wide() + n16)) return st;
+  for (int f = 0; f < b->ds->F; f++) {   // the 16-bit columns with more than 256 bins
+    if (b->codes16[f] == nullptr) continue;
+    const ColumnResult& r = b->results[f];
+    if (int st = ygg_internal_attach_wide_discretized(b->ds, f, b->codes16[f], r.st.num_boundaries + 1, r.st.na_bin)) return st;
+    drop_codes16(b, f);
+  }
   *out = b->ds;
   b->ds = nullptr;  // ownership moves to the caller
   free_builder(b);

@@ -105,36 +105,11 @@ int gen_boundaries(const std::vector<std::pair<float, int64_t>>& cand, int32_t m
   return YGG_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-int ygg_gen_discretized_boundaries(const float* values, const int64_t* counts, int64_t n_candidates,
-                                   int32_t maximum_num_bins, int32_t min_obs_in_bins, const float* special_values,
-                                   int32_t n_special, float* out_boundaries, int32_t capacity,
-                                   int32_t* out_num_boundaries) {
-  if ((n_candidates > 0 && (!values || !counts)) || !out_num_boundaries || (n_special > 0 && !special_values))
-    return YGG_ERR_INVALID_ARGUMENT;
-  if (maximum_num_bins < 1 || maximum_num_bins > 65534 || min_obs_in_bins < 1 || n_candidates < 0 || n_special < 0)
-    return YGG_ERR_INVALID_ARGUMENT;
-  std::vector<std::pair<float, int64_t>> cand(n_candidates);
-  for (int64_t i = 0; i < n_candidates; i++) {
-    if (counts[i] < 1 || (i > 0 && !(values[i] > values[i - 1]))) return YGG_ERR_INVALID_ARGUMENT;
-    cand[i] = {values[i], counts[i]};
-  }
-  std::vector<float> bounds;
-  gen_boundaries(cand, maximum_num_bins, min_obs_in_bins, special_values, n_special, &bounds);
-  *out_num_boundaries = static_cast<int32_t>(bounds.size());
-  if (static_cast<int32_t>(bounds.size()) > capacity || (!out_boundaries && !bounds.empty())) return YGG_ERR_INVALID_ARGUMENT;
-  if (!bounds.empty()) std::memcpy(out_boundaries, bounds.data(), bounds.size() * sizeof(float));
-  return YGG_OK;
-}
-
-int ygg_discretize_boundaries(const float* values, int64_t n, int32_t maximum_num_bins,
-                              int32_t min_obs_in_bins, float* out_boundaries, int32_t capacity,
-                              int32_t* out_num_boundaries, double* out_mean) {
+// ygg_discretize_boundaries(16) once maximum_num_bins is checked: sort + unique + gen_boundaries with {0, mean}.
+int discretize_column(const float* values, int64_t n, int32_t maximum_num_bins, int32_t min_obs_in_bins,
+                      float* out_boundaries, int32_t capacity, int32_t* out_num_boundaries, double* out_mean) {
   if (!values || !out_boundaries || !out_num_boundaries || !out_mean) return YGG_ERR_INVALID_ARGUMENT;
-  if (maximum_num_bins < 2 || maximum_num_bins > 65534 || min_obs_in_bins < 1) return YGG_ERR_INVALID_ARGUMENT;
+  if (min_obs_in_bins < 1) return YGG_ERR_INVALID_ARGUMENT;
   // Non-missing values, their mean (numerical().mean(), data_spec_inference.cc:255-262).
   std::vector<float> v;
   v.reserve(n);
@@ -163,6 +138,47 @@ int ygg_discretize_boundaries(const float* values, int64_t n, int32_t maximum_nu
   if (static_cast<int32_t>(bounds.size()) > capacity) return YGG_ERR_INVALID_ARGUMENT;
   std::memcpy(out_boundaries, bounds.data(), bounds.size() * sizeof(float));
   return YGG_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ygg_gen_discretized_boundaries(const float* values, const int64_t* counts, int64_t n_candidates,
+                                   int32_t maximum_num_bins, int32_t min_obs_in_bins, const float* special_values,
+                                   int32_t n_special, float* out_boundaries, int32_t capacity,
+                                   int32_t* out_num_boundaries) {
+  if ((n_candidates > 0 && (!values || !counts)) || !out_num_boundaries || (n_special > 0 && !special_values))
+    return YGG_ERR_INVALID_ARGUMENT;
+  if (maximum_num_bins < 1 || maximum_num_bins > 65534 || min_obs_in_bins < 1 || n_candidates < 0 || n_special < 0)
+    return YGG_ERR_INVALID_ARGUMENT;
+  std::vector<std::pair<float, int64_t>> cand(n_candidates);
+  for (int64_t i = 0; i < n_candidates; i++) {
+    if (counts[i] < 1 || (i > 0 && !(values[i] > values[i - 1]))) return YGG_ERR_INVALID_ARGUMENT;
+    cand[i] = {values[i], counts[i]};
+  }
+  std::vector<float> bounds;
+  gen_boundaries(cand, maximum_num_bins, min_obs_in_bins, special_values, n_special, &bounds);
+  *out_num_boundaries = static_cast<int32_t>(bounds.size());
+  if (static_cast<int32_t>(bounds.size()) > capacity || (!out_boundaries && !bounds.empty())) return YGG_ERR_INVALID_ARGUMENT;
+  if (!bounds.empty()) std::memcpy(out_boundaries, bounds.data(), bounds.size() * sizeof(float));
+  return YGG_OK;
+}
+
+int ygg_discretize_boundaries(const float* values, int64_t n, int32_t maximum_num_bins,
+                              int32_t min_obs_in_bins, float* out_boundaries, int32_t capacity,
+                              int32_t* out_num_boundaries, double* out_mean) {
+  if (maximum_num_bins < 2 || maximum_num_bins > 65534) return YGG_ERR_INVALID_ARGUMENT;
+  return discretize_column(values, n, maximum_num_bins, min_obs_in_bins, out_boundaries, capacity, out_num_boundaries,
+                           out_mean);
+}
+
+int ygg_discretize_boundaries16(const float* values, int64_t n, int32_t maximum_num_bins,
+                                int32_t min_obs_in_bins, float* out_boundaries, int32_t capacity,
+                                int32_t* out_num_boundaries, double* out_mean) {
+  if (maximum_num_bins < 2 || maximum_num_bins > 65535) return YGG_ERR_INVALID_ARGUMENT;
+  return discretize_column(values, n, maximum_num_bins, min_obs_in_bins, out_boundaries, capacity, out_num_boundaries,
+                           out_mean);
 }
 
 int ygg_discretize_encode(const float* values, int64_t n, const float* boundaries, int32_t num_boundaries,

@@ -184,6 +184,7 @@ struct ygg_gbt {
   float* d_wide_thr = nullptr;       // [split-level nodes][f_scan]
   int32_t* d_wide_feature = nullptr; // [wide features]
   int32_t* d_wide_bins = nullptr;
+  int32_t* d_wide_disc = nullptr;    // [wide features] 1: discretized threshold rule (null without such columns)
   // wide categorical columns (DESIGN.md §21): per-feature tables, the level's positive sets [split-level nodes][n_wide]
   // [set_words], the scan's sort scratch, and the positive-set pool [tree capacity + 1][max_nodes][set_words] (the last
   // tree is d_nodes_scratch's)
@@ -754,8 +755,8 @@ int allocate_wide_buffers(ygg_gbt* h) {
     dev_free(h->d_wnode_sum[i]); dev_free(h->d_wnode_cnt[i]); dev_free(h->d_wnode_hsum[i]);
     h->d_wnode_sum[i] = nullptr; h->d_wnode_cnt[i] = nullptr; h->d_wnode_hsum[i] = nullptr;
   }
-  dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins);
-  h->d_wide_thr = nullptr; h->d_wide_feature = nullptr; h->d_wide_bins = nullptr;
+  dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins); dev_free(h->d_wide_disc);
+  h->d_wide_thr = nullptr; h->d_wide_feature = nullptr; h->d_wide_bins = nullptr; h->d_wide_disc = nullptr;
   dev_free(h->d_wide_cat); dev_free(h->d_wide_na_bin); dev_free(h->d_wide_set); dev_free(h->d_sort_key); dev_free(h->d_sort_idx);
   h->d_wide_cat = nullptr; h->d_wide_na_bin = nullptr; h->d_wide_set = nullptr; h->d_sort_key = nullptr; h->d_sort_idx = nullptr;
   dev_free(h->d_sort_off); h->d_sort_off = nullptr;
@@ -792,6 +793,10 @@ int allocate_wide_buffers(ygg_gbt* h) {
   YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_bins, ds->n_wide()));
   YGG_CUDA(cudaMemcpy(h->d_wide_feature, ds->wide_feature.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
   YGG_CUDA(cudaMemcpy(h->d_wide_bins, ds->wide_bins.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+  if (std::find(ds->wide_disc.begin(), ds->wide_disc.end(), 1) != ds->wide_disc.end()) {
+    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_disc, ds->n_wide()));
+    YGG_CUDA(cudaMemcpy(h->d_wide_disc, ds->wide_disc.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
+  }
   if (h->set_words > 0) {
     // wide categorical columns: (nodes x n_wide x set_words) x 4 B of positive sets, and (slots x sum of sort_pad(B_w)) x 12 B
     // of sort scratch (sort_pad(B) = the power of two >= B, per column)
@@ -809,12 +814,13 @@ int allocate_wide_buffers(ygg_gbt* h) {
                        (static_cast<double>(nodes) * ds->n_wide() * h->set_words * 4 + static_cast<double>(scratch) * 12) / 1e9);
     }
     YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_cat, ds->n_wide()));
-    YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_na_bin, ds->n_wide()));
     YGG_RETURN_IF_ERROR(dev_alloc(&h->d_sort_off, ds->n_wide()));
     YGG_CUDA(cudaMemcpy(h->d_sort_off, sort_off.data(), sizeof(int64_t) * ds->n_wide(), cudaMemcpyHostToDevice));
     YGG_CUDA(cudaMemcpy(h->d_wide_cat, ds->wide_cat.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
-    YGG_CUDA(cudaMemcpy(h->d_wide_na_bin, ds->wide_na_bin.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
   }
+  // the NA bucket of every wide column: a wide categorical split's NA side, a discretized one's na_value
+  YGG_RETURN_IF_ERROR(dev_alloc(&h->d_wide_na_bin, ds->n_wide()));
+  YGG_CUDA(cudaMemcpy(h->d_wide_na_bin, ds->wide_na_bin.data(), sizeof(int32_t) * ds->n_wide(), cudaMemcpyHostToDevice));
   return YGG_OK;
 }
 
@@ -1392,7 +1398,7 @@ int grow_tree(ygg_gbt* h, NodeRec* nodes) {
         wp.slot_sum = h->d_wsum; wp.slot_cnt = h->d_wcnt; wp.slot_hsum = h->d_whsum;
         wp.node_sum = h->d_wnode_sum[par]; wp.node_cnt = h->d_wnode_cnt[par]; wp.node_hsum = h->d_wnode_hsum[par];
         wp.pnode_sum = h->d_wnode_sum[par ^ 1]; wp.pnode_cnt = h->d_wnode_cnt[par ^ 1]; wp.pnode_hsum = h->d_wnode_hsum[par ^ 1];
-        wp.thr_value = h->d_wide_thr;
+        wp.thr_value = h->d_wide_thr; wp.wide_disc = h->d_wide_disc;
         wp.wide_cat = h->d_wide_cat; wp.n_wide = ds->n_wide(); wp.set_words = h->set_words; wp.set_out = h->d_wide_set;
         wp.sort_key = h->d_sort_key; wp.sort_idx = h->d_sort_idx; wp.sort_off = h->d_sort_off; wp.sort_total = h->sort_total;
         const dim3 wgrid(level_slot_bound(h, l), ds->n_wide());
@@ -2513,10 +2519,17 @@ namespace {
 // The byte column of a feature held elsewhere (wide or presorted): a filler over all 256 bins with one bucket, i.e. never
 // a valid split for k_scan.  (All rows in one bin would be as good for the scan, but would push k_hist's packed layout,
 // whose bins take at most 8191 rows per work item, to its slower carry layout.)
+__global__ void __launch_bounds__(256) k_filler(uint8_t* __restrict__ col, int64_t n) {
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; r < n; r += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    col[r] = static_cast<uint8_t>(r & 0xFF);
+}
+
 int set_filler_column(ygg_dataset* ds, int32_t feature) {
-  std::vector<uint8_t> filler(ds->n);
-  for (int64_t r = 0; r < ds->n; r++) filler[r] = static_cast<uint8_t>(r & 0xFF);
-  YGG_CUDA(cudaMemcpy(ds->d_bins + static_cast<int64_t>(feature) * ds->n_pad, filler.data(), ds->n, cudaMemcpyHostToDevice));
+  if (ds->n > 0) {
+    k_filler<<<static_cast<unsigned>(std::min<int64_t>((ds->n + 255) / 256, 4096)), 256>>>(
+        ds->d_bins + static_cast<int64_t>(feature) * ds->n_pad, ds->n);
+    YGG_CUDA(cudaGetLastError());
+  }
   dev_free(ds->d_bins4);   // k_hist2's interleaved copy and k_hist_seg's row-major copy are rebuilt on first use
   ds->d_bins4 = nullptr;
   dev_free(ds->d_bins_rows);
@@ -2526,11 +2539,13 @@ int set_filler_column(ygg_dataset* ds, int32_t feature) {
   return ygg_internal_dataset_finalize(ds);
 }
 
-// The dataset checks and the upload shared by the wide numerical and the wide categorical columns (`values` null:
-// categorical; its bucket values are zeros).
+// The dataset checks and the upload shared by the wide numerical, categorical and discretized columns (`values` null:
+// categorical or discretized, whose bucket values are zeros that nothing reads).  `codes` is host memory, or device
+// memory with `codes_kind` = cudaMemcpyDeviceToDevice.
 int attach_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins, int32_t na_bin,
-                       const float* values, float na_replacement) {
-  const bool categorical = values == nullptr;
+                       const float* values, float na_replacement, bool discretized = false,
+                       cudaMemcpyKind codes_kind = cudaMemcpyHostToDevice) {
+  const bool categorical = values == nullptr && !discretized;
   if (!ds) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (feature < 0 || feature >= ds->F) return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d out of range", feature);
   if (ds->handles > 0)
@@ -2545,13 +2560,8 @@ int attach_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, 
   YGG_RETURN_IF_ERROR(require_device());
   YGG_CUDA(cudaSetDevice(ds->device));
   const int W = ds->n_wide();
-  // the code matrix grows by one plane (the old planes are copied over)
-  uint16_t* grown = nullptr;
-  YGG_RETURN_IF_ERROR(dev_alloc(&grown, static_cast<size_t>(W + 1) * ds->n_pad));
-  if (W > 0) YGG_CUDA(cudaMemcpy(grown, ds->d_wide, sizeof(uint16_t) * W * ds->n_pad, cudaMemcpyDeviceToDevice));
-  YGG_CUDA(cudaMemcpy(grown + static_cast<size_t>(W) * ds->n_pad, codes, sizeof(uint16_t) * n, cudaMemcpyHostToDevice));
-  dev_free(ds->d_wide);
-  ds->d_wide = grown;
+  YGG_RETURN_IF_ERROR(ygg_internal_reserve_wide(ds, W + 1));
+  YGG_CUDA(cudaMemcpy(ds->d_wide + static_cast<size_t>(W) * ds->n_pad, codes, sizeof(uint16_t) * n, codes_kind));
   YGG_RETURN_IF_ERROR(set_filler_column(ds, feature));
   if (ds->wide_of.empty()) { ds->wide_of.assign(ds->F, -1); ds->wide_off.assign(1, 0); }
   ds->wide_of[feature] = W;
@@ -2559,8 +2569,9 @@ int attach_wide_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, 
   ds->wide_bins.push_back(num_bins);
   ds->wide_na_bin.push_back(na_bin);
   ds->wide_cat.push_back(categorical ? 1 : 0);
+  ds->wide_disc.push_back(discretized ? 1 : 0);
   ds->wide_na_replacement.push_back(na_replacement);
-  if (categorical) ds->wide_values.insert(ds->wide_values.end(), static_cast<size_t>(num_bins), 0.f);
+  if (values == nullptr) ds->wide_values.insert(ds->wide_values.end(), static_cast<size_t>(num_bins), 0.f);
   else ds->wide_values.insert(ds->wide_values.end(), values, values + num_bins);
   ds->wide_off.push_back(ds->wide_off.back() + num_bins);
   YGG_RETURN_IF_ERROR(upload_wide_meta(ds));
@@ -2602,6 +2613,38 @@ int ygg_dataset_set_wide_categorical_column(ygg_dataset* ds, int32_t feature, co
   YGG_RETURN_IF_ERROR(check_wide_codes(feature, codes, n, num_bins, na_bin));
   return attach_wide_column(ds, feature, codes, n, num_bins, na_bin, nullptr, 0.f);
 }
+
+int ygg_dataset_set_wide_discretized_column(ygg_dataset* ds, int32_t feature, const uint16_t* codes, int64_t n, int32_t num_bins,
+                                            int32_t na_bin) {
+  YGG_RETURN_IF_ERROR(check_wide_codes(feature, codes, n, num_bins, na_bin));
+  return attach_wide_column(ds, feature, codes, n, num_bins, na_bin, nullptr, 0.f, true);
+}
+
+}  // extern "C"
+
+int ygg_internal_reserve_wide(ygg_dataset* ds, int planes) {
+  if (planes <= ds->wide_cap) return YGG_OK;
+  YGG_CUDA(cudaSetDevice(ds->device));
+  uint16_t* grown = nullptr;   // the old planes are copied over
+  YGG_RETURN_IF_ERROR(dev_alloc(&grown, static_cast<size_t>(planes) * ds->n_pad));
+  if (ds->n_wide() > 0)
+    YGG_CUDA(cudaMemcpy(grown, ds->d_wide, sizeof(uint16_t) * ds->n_wide() * ds->n_pad, cudaMemcpyDeviceToDevice));
+  dev_free(ds->d_wide);
+  ds->d_wide = grown;
+  ds->wide_cap = planes;
+  return YGG_OK;
+}
+
+int ygg_internal_attach_wide_discretized(ygg_dataset* ds, int32_t feature, const uint16_t* d_codes, int32_t num_bins,
+                                         int32_t na_bin) {
+  if (num_bins < kMaxBins + 1 || num_bins > 65535 || na_bin < 0 || na_bin >= num_bins)
+    return set_error(YGG_ERR_INVALID_ARGUMENT, "feature %d: num_bins=%d / na_bin=%d outside [257, 65535] / [0, num_bins)",
+                     feature, num_bins, na_bin);
+  return attach_wide_column(ds, feature, d_codes, ds ? ds->n : 0, num_bins, na_bin, nullptr, 0.f, true,
+                            cudaMemcpyDeviceToDevice);
+}
+
+extern "C" {
 
 int ygg_dataset_get_wide_column(const ygg_dataset* ds, int32_t feature, uint16_t* codes, int32_t* num_bins, int32_t* na_bin) {
   if (!ds || !codes) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
@@ -2873,7 +2916,7 @@ int ygg_gbt_destroy(ygg_gbt* h) {
   dev_free(h->d_goss_u);
   dev_free(h->d_wsum); dev_free(h->d_wcnt); dev_free(h->d_whsum);
   for (int i = 0; i < 2; i++) { dev_free(h->d_wnode_sum[i]); dev_free(h->d_wnode_cnt[i]); dev_free(h->d_wnode_hsum[i]); }
-  dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins);
+  dev_free(h->d_wide_thr); dev_free(h->d_wide_feature); dev_free(h->d_wide_bins); dev_free(h->d_wide_disc);
   dev_free(h->d_wide_cat); dev_free(h->d_wide_na_bin); dev_free(h->d_wide_set); dev_free(h->d_sort_key); dev_free(h->d_sort_idx);
   dev_free(h->d_sets); dev_free(h->d_sort_off);
   dev_free(h->d_master_val); dev_free(h->d_master_row); dev_free(h->d_ps); dev_free(h->d_ph); dev_free(h->d_presort_temp);
@@ -3240,7 +3283,8 @@ int attach_validation(ygg_gbt* h, const ygg_dataset* valid, int64_t n) {
   if (!h->has_labels) return set_error(YGG_ERR_INVALID_ARGUMENT, "set the training labels first (the initial prediction comes from them)");
   if (valid->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset lives on another device");
   if (valid->F != h->ds->F || valid->num_bins != h->ds->num_bins || valid->feature_type != h->ds->feature_type ||
-      valid->wide_feature != h->ds->wide_feature || valid->wide_bins != h->ds->wide_bins || valid->wide_cat != h->ds->wide_cat)
+      valid->wide_feature != h->ds->wide_feature || valid->wide_bins != h->ds->wide_bins || valid->wide_cat != h->ds->wide_cat ||
+      valid->wide_disc != h->ds->wide_disc)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset does not have the features / binning of the training dataset");
   if (n != valid->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "label count %lld != validation rows %lld", static_cast<long long>(n), static_cast<long long>(valid->n));
   YGG_CUDA(cudaSetDevice(h->ds->device));
@@ -3299,9 +3343,10 @@ int ygg_dataset_split_rows(const ygg_dataset* ds, const uint8_t* select, ygg_dat
     if (ds->n_wide() > 0) {   // the wide columns travel with the rows: codes, bucket values and NA replacements
       ygg_dataset* o = out[k];
       o->wide_of = ds->wide_of; o->wide_feature = ds->wide_feature; o->wide_bins = ds->wide_bins; o->wide_na_bin = ds->wide_na_bin;
-      o->wide_cat = ds->wide_cat;
+      o->wide_cat = ds->wide_cat; o->wide_disc = ds->wide_disc;
       o->wide_off = ds->wide_off; o->wide_values = ds->wide_values; o->wide_na_replacement = ds->wide_na_replacement;
       st = dev_alloc(&o->d_wide, static_cast<size_t>(ds->n_wide()) * o->n_pad);
+      o->wide_cap = ds->n_wide();
       if (st == YGG_OK) st = upload_wide_meta(o);
       if (st == YGG_OK) {
         dim3 wgrid(grid.x, static_cast<unsigned>(ds->n_wide()));
@@ -3687,7 +3732,8 @@ int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   if (!h || !ds || !out) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (ds->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset lives on another device");
   if (ds->F != h->ds->F || ds->num_bins != h->ds->num_bins || ds->feature_type != h->ds->feature_type ||
-      ds->wide_feature != h->ds->wide_feature || ds->wide_bins != h->ds->wide_bins || ds->wide_cat != h->ds->wide_cat)
+      ds->wide_feature != h->ds->wide_feature || ds->wide_bins != h->ds->wide_bins || ds->wide_cat != h->ds->wide_cat ||
+      ds->wide_disc != h->ds->wide_disc)
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset does not have the features / binning of the training dataset");
   if (n != ds->n * h->K) return set_error(YGG_ERR_INVALID_ARGUMENT, "n mismatch (rows x classes expected)");
   YGG_CUDA(cudaSetDevice(h->ds->device));

@@ -26,12 +26,14 @@ struct ygg_dataset {
   // Wide numerical columns (ygg_dataset_set_wide_column, DESIGN.md §20): 257..65535 buckets, uint16 codes.  The feature's
   // byte column in d_bins holds a filler with num_bins[f] = 1, so the byte kernels never split on it.
   uint16_t* d_wide = nullptr;          // [wide features][n_pad] codes, in wide-index order
+  int wide_cap = 0;                    // planes allocated in d_wide (>= wide features)
   int32_t* d_wide_of = nullptr;        // [F] wide index of a feature, -1 for a byte column
   int64_t* d_wide_off = nullptr;       // [wide features] offset of the feature's buckets in d_wide_values / the wide planes
   float* d_wide_values = nullptr;      // [sum of the wide features' buckets] bucket values (ascending per feature)
   // Wide categorical columns (ygg_dataset_set_wide_categorical_column, DESIGN.md §21) share these tables: wide_cat[w] = 1,
-  // and their bucket values are zeros that nothing reads.
-  std::vector<int32_t> wide_of, wide_feature, wide_bins, wide_na_bin, wide_cat;
+  // and their bucket values are zeros that nothing reads.  Discretized wide columns (ygg_dataset_set_wide_discretized_column,
+  // DESIGN.md §25) too: wide_disc[w] = 1, split by the discretized threshold rule (NA rows: wide_na_bin[w] >= threshold).
+  std::vector<int32_t> wide_of, wide_feature, wide_bins, wide_na_bin, wide_cat, wide_disc;
   std::vector<int64_t> wide_off;       // host copy of d_wide_off, plus the total at the end
   std::vector<float> wide_values, wide_na_replacement;
   int n_wide() const { return static_cast<int>(wide_feature.size()); }
@@ -57,3 +59,9 @@ struct ygg_dataset {
 __attribute__((visibility("hidden"))) int ygg_internal_dataset_alloc(ygg_dataset** out, int64_t n_rows,
                                                                      int32_t n_features, int32_t device);
 __attribute__((visibility("hidden"))) int ygg_internal_dataset_finalize(ygg_dataset* ds);
+// Grows d_wide to hold at least `planes` code planes (one allocation for the columns that will be attached).
+__attribute__((visibility("hidden"))) int ygg_internal_reserve_wide(ygg_dataset* ds, int planes);
+// ygg_dataset_set_wide_discretized_column with the codes already on the device (the GPU binning step's output).
+__attribute__((visibility("hidden"))) int ygg_internal_attach_wide_discretized(ygg_dataset* ds, int32_t feature,
+                                                                              const uint16_t* d_codes, int32_t num_bins,
+                                                                              int32_t na_bin);

@@ -804,9 +804,15 @@ struct SelectParams {
   const float* wide_thr_value; // [level nodes][f_count]
   // wide categorical columns: the positive sets k_scan_wide_cat left per (level node, wide feature) (null without them)
   const uint32_t* wide_set;    // [level nodes][n_wide][set_words]
-  const int32_t* wide_na_bin;  // [n_wide]
+  const int32_t* wide_na_bin;  // [n_wide] NA bucket of every wide column (null without wide columns)
   int n_wide, set_words;
 };
+
+// The NA bucket of numerical feature fg: a wide column's own, else its byte column's.
+__device__ __forceinline__ int numerical_na_bin(const SelectParams& p, int fg) {
+  const int wi = p.wide_of != nullptr ? p.wide_of[fg] : -1;
+  return wi >= 0 ? p.wide_na_bin[wi] : p.na_bin[fg];
+}
 
 // Candidate (level node j, wide index wi) is a wide categorical one: its positive set is in p.wide_set.
 __device__ __forceinline__ const uint32_t* wide_set_of(const SelectParams& p, int j, int wi) {
@@ -906,7 +912,7 @@ __global__ void __launch_bounds__(256) k_select_local(SelectParams p) {
               // keeps the engine's choice and counts the node as unresolved when the reference would take it
               if (wide_cat_index(p, fg, 1) >= 0) a.n_pos = -1;
             } else {
-              a.na_value = (p.na_bin[fg] >= a.thr) ? 1 : 0;   // na_bin > thr - 1
+              a.na_value = (numerical_na_bin(p, fg) >= a.thr) ? 1 : 0;   // na_bin > thr - 1
               if (a.thr_value == a.thr_value) a.na_value = p.na_replacement[fg] >= a.thr_value ? 1 : 0;   // exact rule (:218)
             }
             p.ties[j].alt[pos] = a;
@@ -1144,7 +1150,7 @@ __global__ void __launch_bounds__(256) k_select_global(SelectParams p) {
 #pragma unroll
         for (int i = 0; i < 8; i++) nd->mask[i] = best.mask[i];
         nd->na_value = best.cond_type == 1 ? best.na_value
-                                           : ((p.na_bin[best.feature] >= best.thr) ? 1 : 0);  // na_bin > thr - 1
+                                           : ((numerical_na_bin(p, best.feature) >= best.thr) ? 1 : 0);  // na_bin > thr - 1
         // exact rule: na_value = na_replacement >= threshold (splitter_accumulator.h:218)
         if (nd->thr_value == nd->thr_value) nd->na_value = p.na_replacement[best.feature] >= nd->thr_value ? 1 : 0;
         nd->score = best.score;

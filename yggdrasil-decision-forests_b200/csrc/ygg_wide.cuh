@@ -1,7 +1,7 @@
 // ygg_wide.cuh — histogram and scan kernels of the wide numerical columns (DESIGN.md §20).
 //
-// A wide column is a numerical feature with 257..65535 buckets, one per distinct value, stored as uint16 codes in its
-// own matrix (ygg_dataset.d_wide).  Its histograms do not fit k_hist's shared-memory tiles: they live in global memory
+// A wide column is a numerical feature with 257..65535 buckets, one per distinct value (or, discretized, one per bin of
+// the GPU binning step, DESIGN.md §25), stored as uint16 codes in its own matrix (ygg_dataset.d_wide).  Its histograms do not fit k_hist's shared-memory tiles: they live in global memory
 // as [slot][sum over the wide features of B_f] planes, accumulated with 64-bit / 32-bit integer atomics from the same
 // active lists and 24-bit quantised gradients as k_hist's (exact and order independent, DESIGN.md §3), and scanned by
 // one CTA per (family, wide feature) in tiles of 256 buckets with a running carry, scored by boundary_score.
@@ -66,6 +66,7 @@ struct WideScanParams {
   const uint32_t* pnode_cnt;
   const unsigned long long* pnode_hsum;
   float* thr_value;              // [level nodes][f_count] float threshold of the wide candidates (SelectParams.wide_thr_value)
+  const int32_t* wide_disc;      // [wide features] 1: discretized threshold rule (DESIGN.md §25); null without such columns
   // wide categorical columns (k_scan_wide_cat; null / 0 without them)
   const int32_t* wide_cat;       // [wide features] 1: categorical
   int n_wide, set_words;
@@ -92,10 +93,11 @@ __device__ __forceinline__ Scan3 wide_bucket(const WideScanParams& p, size_t d, 
 }
 
 // Scans one node of one wide feature (all 256 threads); thread 0 writes the Candidate and the float threshold.
-// `copy_to` (or null): the node's plane at the level, kept when it is a parent at the next level.
+// `copy_to` (or null): the node's plane at the level, kept when it is a parent at the next level.  `disc`: the column
+// takes the discretized threshold rule (bucket interpolation, no float threshold) instead of §14's exact one.
 template <bool HESS>
 __device__ void scan_wide_node(const WideScanParams& p, int node, int fl, int B, const float* values, size_t d, size_t x,
-                               bool derived, size_t copy_to, bool copy) {
+                               bool derived, size_t copy_to, bool copy, bool disc) {
   __shared__ Scan3 s_warp[8];
   __shared__ double s_best_score[8];
   __shared__ int s_best_b[8];
@@ -170,7 +172,16 @@ __device__ void scan_wide_node(const WideScanParams& p, int node, int fl, int B,
     const size_t ci = static_cast<size_t>(node - lv.first_node) * p.s.f_count + fl;
     Candidate c{0.f, 0, 0, 0};
     float threshold = __builtin_nanf("");
-    if (found) {
+    if (found && disc) {
+      // scan_node's bucket interpolation (splitter_scanner.h:993-1000, :1076-1086): hi is the first non-empty bucket
+      // after the best boundary; the scan visits it only below B - 1
+      int idx = bb;
+      if (s_hi <= B - 2 && s_hi != bb + 1) idx = (bb + s_hi) / 2;
+      c.found = 1;
+      c.score = static_cast<float>(bs);
+      c.thr = idx + 1;
+      c.n_pos = static_cast<int32_t>(s_npos);
+    } else if (found) {
       const int hi = s_hi != 0x7fffffff ? s_hi : bb + 1;
       // §14's exact rule: the middle of the two values present in the node around the cut; the bin threshold is the
       // first bucket whose value reaches it (every bucket in between is empty in this node)
@@ -207,18 +218,19 @@ __global__ void __launch_bounds__(256) k_scan_wide(WideScanParams p) {
   const int B = p.wide_bins[w];
   const int64_t off = p.off[w];
   const float* values = p.values + off;
+  const bool disc = p.wide_disc != nullptr && p.wide_disc[w];
   const NodeRec direct = p.s.nodes[fam.direct];
   const size_t d = static_cast<size_t>(direct.slot) * p.total + off;
   const size_t dn = static_cast<size_t>(fam.direct - lv.first_node) * p.total + off;
   // a node's plane is needed at the next level only if it can be split there
-  if (direct.candidate) scan_wide_node<HESS>(p, fam.direct, fl, B, values, d, 0, false, dn, p.s.write_derived != 0);
+  if (direct.candidate) scan_wide_node<HESS>(p, fam.direct, fl, B, values, d, 0, false, dn, p.s.write_derived != 0, disc);
   if (fam.derived >= 0) {
     const NodeRec derived = p.s.nodes[fam.derived];
     if (derived.candidate) {
       const LevelDesc plv = p.s.levels[p.s.level - 1];
       const size_t x = static_cast<size_t>(fam.parent - plv.first_node) * p.total + off;
       const size_t xn = static_cast<size_t>(fam.derived - lv.first_node) * p.total + off;
-      scan_wide_node<HESS>(p, fam.derived, fl, B, values, d, x, true, xn, p.s.write_derived != 0);
+      scan_wide_node<HESS>(p, fam.derived, fl, B, values, d, x, true, xn, p.s.write_derived != 0, disc);
     }
   }
 }

@@ -33,11 +33,13 @@ class DiscretizedColumn:
     num_missing: int = 0
     num_values: int = 0
     bucket_values: Optional[np.ndarray] = None   # lossless columns: the value of every bucket (exact threshold rule)
+    maximum_num_bins: Optional[int] = None        # the bin budget asked for above 256 (DiscretizedNumericalSpec)
     feature_type = _capi.FEATURE_DISCRETIZED_NUMERICAL
 
     @property
     def wide(self) -> bool:
-        """More buckets than a byte holds: a wide column (uint16 codes, _capi.Dataset.set_wide_column)."""
+        """More buckets than a byte holds: a wide column (uint16 codes, _capi.Dataset.set_wide_column, or without bucket
+        values _capi.Dataset.set_wide_discretized_column)."""
         return self.num_bins > 256
 
     def encode(self, values) -> np.ndarray:
@@ -210,6 +212,22 @@ def infer_column(name: str, values, maximum_num_bins: int = 255, min_obs_in_bins
                              num_missing=int(np.isnan(v).sum()), num_values=len(v))
 
 
+def infer_column16(name: str, values, maximum_num_bins: int, min_obs_in_bins: int = 3,
+                   max_rows: Optional[int] = None) -> DiscretizedColumn:
+    """infer_column for up to 65535 bins: the same rule (GenDiscretizedBoundaries with the special values {0, mean}).  A column that ends with more than 256 bins is a discretized wide column (encode16); one with fewer a
+    byte column, exactly as infer_column would make it."""
+    v = np.asarray(values, dtype=np.float32)
+    sample = v if (max_rows is None or len(v) <= max_rows) else v[:max_rows]
+    boundaries, mean = _capi.discretize_boundaries16(sample, maximum_num_bins, min_obs_in_bins)
+    if len(boundaries) + 1 > 65535:
+        raise ValueError(f"column {name!r}: {len(boundaries) + 1} bins do not fit the engine's uint16 codes")
+    na_bin = int(np.searchsorted(boundaries, np.float32(mean), side="right"))
+    return DiscretizedColumn(name=name, boundaries=boundaries, mean=float(mean),
+                             num_bins=len(boundaries) + 1, na_bin=na_bin,
+                             num_missing=int(np.isnan(v).sum()), num_values=len(v),
+                             maximum_num_bins=int(maximum_num_bins) if maximum_num_bins > 256 else None)
+
+
 def infer_column_lossless(name: str, values, max_rows: Optional[int] = None,
                           max_distinct: int = 255) -> Optional[DiscretizedColumn]:
     """One bin per distinct value, for a numerical column with at most 255 of them (None otherwise).
@@ -285,8 +303,8 @@ def encode_features(cols: Dict[str, np.ndarray], columns: Sequence[DiscretizedCo
 
 def device_dataset(bins: np.ndarray, columns: Sequence, device: int = 0) -> "_capi.Dataset":
     """The device dataset of encode_features' output: byte columns as they are, wide columns (more than 256 buckets)
-    attached with their codes (and, numerical, their bucket values and mean), presorted numerical columns with their
-    values and mean."""
+    attached with their codes (and, exact numerical, their bucket values and mean), presorted numerical columns with
+    their values and mean."""
     wide = [i for i, c in enumerate(columns) if _presorted(c) or c.num_bins > 256]
     byte_bins = np.zeros(bins.shape, np.uint8) if bins.dtype != np.uint8 else bins
     if bins.dtype != np.uint8:
@@ -304,6 +322,8 @@ def device_dataset(bins: np.ndarray, columns: Sequence, device: int = 0) -> "_ca
                 ds.set_numerical_column(i, bins[i], c.mean)
             elif c.feature_type == _capi.FEATURE_CATEGORICAL:
                 ds.set_wide_categorical_column(i, bins[i], c.num_bins, c.na_bin)
+            elif c.bucket_values is None:   # discretized: no bucket values
+                ds.set_wide_discretized_column(i, bins[i], c.num_bins, c.na_bin)
             else:
                 ds.set_wide_column(i, bins[i], c.num_bins, c.na_bin, c.bucket_values, c.mean)
     except Exception:

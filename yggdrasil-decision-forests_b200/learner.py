@@ -187,8 +187,10 @@ class GradientBoostedTreesLearner:
             self.loss = "SQUARED_ERROR"
         else:
             raise NotImplementedError(f"task {task} is outside the accelerated path")
-        if not (2 <= self.num_discretized_numerical_bins <= 256):
-            raise ValueError("num_discretized_numerical_bins must be in [2, 256] (uint8 bins)")
+        # up to 256 bins: byte columns; above, columns with more than 256 bins become discretized wide columns (uint16 codes,
+        # DESIGN.md §25), whose histogram memory grows with their bins
+        if not (2 <= self.num_discretized_numerical_bins <= 65535):
+            raise ValueError("num_discretized_numerical_bins must be in [2, 65535] (uint16 bins)")
         self.cfg = _capi.default_config(
             loss=_LOSS_ID.get(self.loss, 0), num_trees=int(num_trees), shrinkage=float(shrinkage),
             max_depth=int(max_depth), min_examples=int(min_examples),
@@ -291,14 +293,16 @@ class GradientBoostedTreesLearner:
                 else:
                     stats = 0 if self.max_rows_stats is None else min(int(self.max_rows_stats), n)
                     # enqueued: the upload of this column overlaps the sort / boundary kernels of the previous ones
-                    builder.add_numerical_async(f, np.asarray(v, dtype=np.float32),
-                                                self.num_discretized_numerical_bins, 3, n_stats_rows=stats)
+                    add = builder.add_numerical_async if self.num_discretized_numerical_bins <= 256 else \
+                        builder.add_numerical16_async
+                    add(f, np.asarray(v, dtype=np.float32), self.num_discretized_numerical_bins, 3, n_stats_rows=stats)
                     pending.append((f, name))
             for f, name in pending:
                 bounds, mean, na_bin, missing = builder.get_numerical(f)
-                columns[f] = ds_lib.DiscretizedColumn(name=name, boundaries=bounds, mean=float(mean),
-                                                      num_bins=len(bounds) + 1, na_bin=na_bin,
-                                                      num_missing=int(missing), num_values=n)
+                columns[f] = ds_lib.DiscretizedColumn(
+                    name=name, boundaries=bounds, mean=float(mean), num_bins=len(bounds) + 1, na_bin=na_bin,
+                    num_missing=int(missing), num_values=n,
+                    maximum_num_bins=self.num_discretized_numerical_bins if self.num_discretized_numerical_bins > 256 else None)
             dataset = builder.finish()
             for f, c in enumerate(columns):
                 if c.feature_type == _capi.FEATURE_CATEGORICAL and c.wide:

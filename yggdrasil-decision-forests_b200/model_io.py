@@ -128,8 +128,12 @@ def encode_data_spec(spec) -> (bytes, int, List[int]):
         if len(c.boundaries):
             num += pb_f32(2, float(c.boundaries[0])) + pb_f32(3, float(c.boundaries[-1]))
         disc = pb_bytes(1, np.asarray(c.boundaries, dtype="<f4").tobytes())  # packed repeated float
-        # maximum_num_bins: 255 for the discretized and byte lossless columns; a wide column's own bucket count
-        disc += pb_int(3, max(255, len(c.boundaries) + 1) if c.num_bins > 256 else 255) + pb_int(4, 3)
+        # maximum_num_bins: the budget asked for above 256 bins; else 255 for the discretized and byte lossless columns
+        # and a wide lossless column's own bucket count
+        budget = getattr(c, "maximum_num_bins", None)
+        if budget is None:
+            budget = max(255, len(c.boundaries) + 1) if c.num_bins > 256 else 255
+        disc += pb_int(3, budget) + pb_int(4, 3)
         col = pb_int(1, 9) + pb_bytes(2, c.name) + pb_int(3, 0) + pb_bytes(5, num)  # DISCRETIZED_NUMERICAL
         col += pb_int(7, c.num_missing) + pb_bytes(8, disc)
         cols.append(col)
