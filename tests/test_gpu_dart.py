@@ -35,9 +35,12 @@ def gradients(loss, s, labels):
     return g[None], h[None], g[None], h[None]
 
 
-def check_dart_run(gbt, cfg, table, labels, rate, iters, vlabels=None, weights=None):
+def check_dart_run(gbt, cfg, table, labels, rate, iters, vlabels=None, weights=None, vweights=None, on_tree=None):
     """`cfg.candidate_shuffle` 1 / 2 takes trees of depth 2 (max_depth = 2): exactly one candidate shuffle per tree, at
-    its root, which the restatement replays on the learner's stream after the iteration's DART and row draws."""
+    its root, which the restatement replays on the learner's stream after the iteration's DART and row draws.
+    vweights: the held-out rows' weights.  on_tree(t, rows): called after each tree's checks, before the next step(),
+    with the per-row quantities the tree was trained on (dict g, h, g_alt, h_alt, sel, w, tree, as check_run hands
+    them out), taken at the sampled predictions."""
     n = table.n
     shuffle = int(cfg.candidate_shuffle)
     assert shuffle == 0 or int(cfg.max_depth) == 2
@@ -98,6 +101,9 @@ def check_dart_run(gbt, cfg, table, labels, rate, iters, vlabels=None, weights=N
                           w=w if weighted else None, w_pow2=w_pow2, g2w=g2w, g2w_alt=g2w_alt)
             rows_of = R.route(tree, table.cols, sets)
             errs += R.check_tree(tree, rows_of, rows, cfg, logit, where=f"tree {t}")
+            if on_tree is not None:
+                on_tree(t, dict(g=gk, h=hk if has_h else None, g_alt=gk_alt, h_alt=hk_alt if has_h else None, sel=sel,
+                                w=w if weighted else None, tree=tree))
             if shuffle == 1:
                 rng.shuffle(len(table.cols))
             elif shuffle == 2:
@@ -121,7 +127,8 @@ def check_dart_run(gbt, cfg, table, labels, rate, iters, vlabels=None, weights=N
         errs += check_losses(gbt.train_loss(it), loss, acc.acc, labels, weights,
                              w_pow2 if weights is not None else None, f"train loss {it}")
         if vacc is not None:
-            errs += check_losses(gbt.validation_loss(it), loss, vacc.acc, np.asarray(vlabels), None, None,
+            vw_pow2 = R.pow2_cover(np.max(vweights)) if vweights is not None else None
+            errs += check_losses(gbt.validation_loss(it), loss, vacc.acc, np.asarray(vlabels), vweights, vw_pow2,
                                  f"validation loss {it}")
     # the model: every leaf of iteration j scaled by w_j, summed in tree order
     want = D.scaled_sum(init, np.stack(leaves), acc.weights(), K)

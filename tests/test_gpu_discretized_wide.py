@@ -502,6 +502,49 @@ def test_dart_matches_oracle(loss, rate, policy):
         d.close()
 
 
+def test_builder_dataset_takes_a_held_out_dataset_made_in_feature_order():
+    """The GPU binning step attaches its 16-bit columns when the builder finishes, so a wide column set on the finished
+    dataset comes after them in its wide order.  A held-out dataset made column by column in feature order has the
+    same features: set_validation and predict() accept it and route its rows by its own codes; a dataset whose wide
+    column at a feature is of another kind is still refused."""
+    from tests import boost_ref as R
+    rng = np.random.default_rng(61)
+    n, nv = 20000, 3000
+    x = rng.normal(size=n + nv).astype(np.float32)
+    codes = rng.integers(0, 600, size=n + nv).astype(np.uint16)
+    values = np.arange(600, dtype=np.float32)
+    b = ydf_b200.DatasetBuilder(n, 2)
+    b.add_bins(0, np.zeros(n, np.uint8), 1, 0)
+    b.add_numerical16_async(1, x[:n], 4096, 3)
+    col = dataspec.infer_column16("x", x[:n], 4096)
+    ds = b.finish()
+    ds.set_wide_column(0, codes[:n], 600, 0, values, 0.0)
+    assert col.wide and ds.wide == {1: (col.num_bins, col.na_bin), 0: (600, 0)}
+    enc = col.encode16(x[n:])
+    va = ydf_b200.Dataset(np.zeros((2, nv), np.uint8), [1, 1], [0, 0])
+    va.set_wide_column(0, codes[n:], 600, 0, values, 0.0)
+    va.set_wide_discretized_column(1, enc, col.num_bins, col.na_bin)
+    y = ((np.sin(2 * x) + codes / 300.0 + rng.normal(scale=0.3, size=n + nv)) > 1).astype(np.int32) + 1
+    gbt = ydf_b200.Gbt(ds, ydf_b200.default_config(max_depth=4, num_trees=3))
+    gbt.set_labels(y[:n])
+    gbt.set_validation(va, y[n:])
+    gbt.train(3)
+    cols = [("wide_num", codes[n:], 600, values), ("wide_num", enc, col.num_bins, None)]
+    want = np.full(nv, np.float32(gbt.initial_prediction()), np.float32)
+    for t in range(3):
+        tree = gbt.get_tree(t)
+        want = (want + tree["leaf_value"][R.leaf_of_rows(tree, R.route(tree, cols), nv)]).astype(np.float32)
+    assert {0, 1} <= set(np.concatenate([gbt.get_tree(t)["feature"] for t in range(3)]).tolist())
+    assert np.array_equal(gbt.predict(va), want)
+    other = ydf_b200.Dataset(np.zeros((2, nv), np.uint8), [1, 1], [0, 0])
+    other.set_wide_column(0, codes[n:], 600, 0, values, 0.0)
+    other.set_wide_column(1, enc, col.num_bins, 0, np.arange(col.num_bins, dtype=np.float32), 0.0)
+    with pytest.raises(ydf_b200.YggError, match="features / binning"):
+        gbt.predict(other)
+    for d in (gbt, ds, va, other):
+        d.close()
+
+
 # ---- mixed with wide categorical and presorted columns; candidate sampling ---------------------------------------------
 
 def mixed_wide(rng, n):

@@ -92,9 +92,9 @@ def _weights(rng, m):
 class Case:
     """A draw's data, labels and weights, and the handles trained on them."""
 
-    def __init__(self, d):
+    def __init__(self, d, table=None):
         self.d = d
-        self.table = FuzzTable(d)
+        self.table = FuzzTable(d) if table is None else table
         rng = np.random.default_rng([d["seed"], 2])
         m = self.table.margin(rng, d["scale"])
         if d["scale"] >= 1e3:
@@ -138,8 +138,22 @@ def run_case(seed):
 
 def _plain_case(case, stats):
     d, table = case.d, case.table
-    capture = D.capture_allowed(d)
     gbt, cfg = case.handle()
+    checked, _ = check_run(gbt, cfg, table, case.y, case.vy, weights=case.w, iters=d["iters"],
+                           step=d["drive"] == "step", vweights=case.vw, on_tree=scan_checker(gbt, cfg, d, table, stats))
+    stats["nodes"] += checked
+    check_skipped_share(stats)
+    if d["n_valid"]:
+        # without early stopping the model is whole: the last iteration's loss, not triggered
+        got = gbt.final_validation()
+        assert got == (gbt.validation_loss(d["iters"] - 1)[0], False), got
+    return gbt
+
+
+def scan_checker(gbt, cfg, d, table, stats):
+    """The on_tree callback of check_run (and tests/test_gpu_dart.check_dart_run) that checks the captured candidates
+    of the draw's trees against the exact scan, where the draw allows the capture (which it turns on)."""
+    capture = D.capture_allowed(d)
     K = d["K"]
     kv = k_valid(cfg, d["F"], *d["candidates"]) if d["candidates"] is not None else None
     sampled = kv is not None and CS.num_candidate_attributes(d["F"], cfg.loss, *d["candidates"]) < d["F"]
@@ -172,15 +186,12 @@ def _plain_case(case, stats):
                                        w=rows["w"], trained_tree=True)
             stats["flags"] += flags
 
-    checked, _ = check_run(gbt, cfg, table, case.y, case.vy, weights=case.w, iters=d["iters"],
-                           step=d["drive"] == "step", vweights=case.vw, on_tree=on_tree)
-    stats["nodes"] += checked
+    return on_tree
+
+
+def check_skipped_share(stats):
     if stats["scan_trees"] + stats["skipped"]:
         assert stats["skipped"] <= MAX_SKIPPED_SHARE * (stats["scan_trees"] + stats["skipped"]), stats
-    if d["n_valid"]:
-        # without early stopping the model is whole: the last iteration's loss, not triggered
-        got = gbt.final_validation()
-        assert got == (gbt.validation_loss(d["iters"] - 1)[0], False), got
 
 
 def _early_stopping_case(case, stats):
@@ -210,6 +221,7 @@ def _early_stopping_case(case, stats):
                            trained=True, logged=logged, kept_trees=want["kept_trees"],
                            on_tree=lambda t, rows: stats.__setitem__("trees", stats["trees"] + 1))
     stats["nodes"] += checked
+    return gbt
 
 
 # what a rename may change: the whole condition, its kind included (on a small node a numerical column can send the
@@ -259,6 +271,7 @@ def _replay_case(case, stats):
         assert ties == (n_renamed, n_unresolved), (ties, n_renamed, n_unresolved)
     stats["renamed"] += ties[0]
     stats["unresolved"] += ties[1]
+    return gbt
 
 
 def _tie_candidates(gbt, cfg, tree, t, table):

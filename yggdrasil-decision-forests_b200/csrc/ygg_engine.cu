@@ -3276,15 +3276,29 @@ int alloc_dart_history(ygg_gbt* h, uint16_t** p, int64_t rows, const char* what)
   return YGG_OK;
 }
 
+// The features and binning of dataset `a` are those of `b`: per feature its buckets and type, and for a wide column its
+// bucket count and kind.  The wide index is the order the columns were attached in (the GPU binning step attaches its
+// 16-bit columns at finish, after any set earlier), so two datasets are compared feature by feature, not by index.
+bool same_features(const ygg_dataset* a, const ygg_dataset* b) {
+  if (a->F != b->F || a->num_bins != b->num_bins || a->feature_type != b->feature_type || a->n_wide() != b->n_wide())
+    return false;
+  for (int f = 0; f < a->F && a->n_wide() > 0; f++) {
+    const int wa = a->wide_of[f], wb = b->wide_of[f];
+    if ((wa >= 0) != (wb >= 0)) return false;
+    if (wa >= 0 && (a->wide_bins[wa] != b->wide_bins[wb] || a->wide_cat[wa] != b->wide_cat[wb] ||
+                    a->wide_disc[wa] != b->wide_disc[wb]))
+      return false;
+  }
+  return true;
+}
+
 int attach_validation(ygg_gbt* h, const ygg_dataset* valid, int64_t n) {
   (void)cudaGetLastError();  // stale foreign error, see ygg_gbt_step
   if (h->trees_done > 0) return set_error(YGG_ERR_INVALID_ARGUMENT, "validation rows must be attached before training");
   if (h->shard_mode != kShardNone) return set_error(YGG_ERR_UNIMPLEMENTED, "validation rows are not combined with sharding");
   if (!h->has_labels) return set_error(YGG_ERR_INVALID_ARGUMENT, "set the training labels first (the initial prediction comes from them)");
   if (valid->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset lives on another device");
-  if (valid->F != h->ds->F || valid->num_bins != h->ds->num_bins || valid->feature_type != h->ds->feature_type ||
-      valid->wide_feature != h->ds->wide_feature || valid->wide_bins != h->ds->wide_bins || valid->wide_cat != h->ds->wide_cat ||
-      valid->wide_disc != h->ds->wide_disc)
+  if (!same_features(valid, h->ds))
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the validation dataset does not have the features / binning of the training dataset");
   if (n != valid->n) return set_error(YGG_ERR_INVALID_ARGUMENT, "label count %lld != validation rows %lld", static_cast<long long>(n), static_cast<long long>(valid->n));
   YGG_CUDA(cudaSetDevice(h->ds->device));
@@ -3731,9 +3745,7 @@ int ygg_gbt_get_predictions(ygg_gbt* h, float* out, int64_t n) {
 int ygg_gbt_predict(ygg_gbt* h, const ygg_dataset* ds, float* out, int64_t n) {
   if (!h || !ds || !out) return set_error(YGG_ERR_INVALID_ARGUMENT, "null argument");
   if (ds->device != h->ds->device) return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset lives on another device");
-  if (ds->F != h->ds->F || ds->num_bins != h->ds->num_bins || ds->feature_type != h->ds->feature_type ||
-      ds->wide_feature != h->ds->wide_feature || ds->wide_bins != h->ds->wide_bins || ds->wide_cat != h->ds->wide_cat ||
-      ds->wide_disc != h->ds->wide_disc)
+  if (!same_features(ds, h->ds))
     return set_error(YGG_ERR_INVALID_ARGUMENT, "the dataset does not have the features / binning of the training dataset");
   if (n != ds->n * h->K) return set_error(YGG_ERR_INVALID_ARGUMENT, "n mismatch (rows x classes expected)");
   YGG_CUDA(cudaSetDevice(h->ds->device));
